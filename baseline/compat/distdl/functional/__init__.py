@@ -3,7 +3,7 @@ import torch
 
 class ZeroVolumeCorrectorFunction(torch.autograd.Function):
     """Loss epilogue: a worker whose loss is zero-volume gets a scalar 0 so that every worker can call
-    ``.backward()``; the backward hands an empty gradient back (``/root/reference/dfno/loss.py:35``)."""
+    ``.backward()``; the backward hands an empty gradient back (reference ``dfno/loss.py:35``)."""
 
     @staticmethod
     def forward(ctx, value):

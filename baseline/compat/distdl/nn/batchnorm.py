@@ -6,7 +6,7 @@ from ..backend.backend import _on
 
 class DistributedBatchNorm(torch.nn.Module):
     """Per-channel batch norm with statistics summed over all workers.  The reference only constructs it
-    (``/root/reference/dfno/dfno.py:325-326``; it is commented out of the forward)."""
+    (reference ``dfno/dfno.py:325-326``; it is commented out of the forward)."""
 
     def __init__(self, P_x, num_features, eps=1e-5, momentum=0.1, affine=True, track_running_stats=True,
                  device=None, dtype=None):

@@ -34,7 +34,7 @@ class _Bcast(torch.autograd.Function):
 
 class Broadcast(torch.nn.Module):
     """``Broadcast(P_root, P_x)``: differentiable copy from a one-worker partition to all workers
-    (``/root/reference/dfno/dfno.py:41-42``).  Adjoint = :class:`SumReduce`."""
+    (reference ``dfno/dfno.py:41-42``).  Adjoint = :class:`SumReduce`."""
 
     def __init__(self, P_x, P_y, **_unused):
         super().__init__()

@@ -1,5 +1,5 @@
 """``Repartition(P_a, P_b)``: move one global tensor from the balanced block decomposition over ``P_a`` to
-the one over ``P_b`` (``/root/reference/dfno/dfno.py:99-102``).  Every pair of workers whose blocks
+the one over ``P_b`` (reference ``dfno/dfno.py:99-102``).  Every pair of workers whose blocks
 overlap exchanges exactly that overlap; here all pairs go out in ONE ``all_to_all_single`` over the
 world group (DistDL posts an Isend/Irecv per pair)."""
 import numpy as np

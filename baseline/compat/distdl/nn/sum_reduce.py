@@ -30,7 +30,7 @@ class _Reduce(torch.autograd.Function):
 
 
 class SumReduce(torch.nn.Module):
-    """``SumReduce(P_x, P_root)`` (``/root/reference/dfno/loss.py:17-18``).  Adjoint = :class:`Broadcast`."""
+    """``SumReduce(P_x, P_root)`` (reference ``dfno/loss.py:17-18``).  Adjoint = :class:`Broadcast`."""
 
     def __init__(self, P_x, P_y, **_unused):
         super().__init__()

@@ -1,5 +1,5 @@
 """``distdl.utilities.torch`` (star-imported by the reference, which relies on ``np`` / ``torch``
-leaking through it: ``/root/reference/dfno/utils.py:8-9,80``)."""
+leaking through it: reference ``dfno/utils.py:8-9,80``)."""
 import numpy as np                                          # noqa: F401
 import torch                                                # noqa: F401
 

@@ -1,8 +1,8 @@
-"""`bench.py --impl reference`: the UNMODIFIED reference (`baseline/_ref/dfno`, installed with pip from
-/root/reference) through its own public API and stock code path --
+"""`bench.py --impl reference`: the UNMODIFIED reference (`baseline/_ref/dfno`, installed with pip from a
+checkout of slimgroup/dfno) through its own public API and stock code path --
 
     dfno.create_standard_partitions -> dfno.DistributedFNO -> dfno.DistributedRelativeLpLoss ->
-    torch.optim.Adam, the loop of /root/reference/training/two_phase/train_two_phase.py:99-117
+    torch.optim.Adam, the loop of the reference's training/two_phase/train_two_phase.py:99-117
 
 -- fp32 (the only dtype the reference supports on GPU, dfno.py:80), same 128^3 x 20 config, same timing
 method as the product arm.  Nothing of `dfno_b200` (models, kernels, engine, communication layer) is
@@ -21,10 +21,12 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 def _import_reference():
     """Returns (dfno module, comm description).  Real DistDL first; the torch.distributed stand-in otherwise."""
-    ref_dir, shim_dir = os.path.join(HERE, "_ref"), os.path.join(HERE, "compat")
-    if not os.path.isdir(os.path.join(ref_dir, "dfno")):
-        raise ImportError("baseline/_ref/dfno is missing: pip install --no-index --no-deps --target baseline/_ref "
-                          "<copy of /root/reference> (DESIGN.md, 'Reference arm')")
+    shim_dir = os.path.join(HERE, "compat")
+    candidates = [os.path.join(HERE, "_ref"), os.path.join(os.path.dirname(HERE), "oracle", "_ref")]
+    ref_dir = next((d for d in candidates if os.path.isdir(os.path.join(d, "dfno"))), None)
+    if ref_dir is None:
+        raise ImportError("the reference package is missing: oracle/install_reference.sh <checkout of slimgroup/dfno> "
+                          "(DESIGN.md, 'Reference arm')")
     for name in [m for m in sys.modules if m == "dfno" or m.startswith("dfno.")]:
         del sys.modules[name]
     sys.path.insert(0, ref_dir)
@@ -148,7 +150,7 @@ def run(args, ClockSampler):
             "config": {"model": f"FNO3d+t {G}^3x{T}t width {args.width} modes {tuple(args.modes)} blocks {args.blocks}",
                        "global_batch": args.batch, "seq_len": G * G * G * T,
                        "parallelism": f"P_x = {grid} (reference planner: P_m, P_y derived by dfno.py:82-97)",
-                       "l2": "per-step working set (GBs of fp32 activations) exceeds the 126 MB L2; no flush needed",
+                       "l2": "per-step working set (GBs of fp32 activations) exceeds the 50 MB L2 of an H100; no flush needed",
                        "step": "forward + DistributedRelativeLpLoss + backward + torch.optim.Adam"},
             "clocks": clocks, "e2e": e2e, "loss": float(last) if last is not None else None,
             "peak_mem_gb": peak / 2 ** 30, "gpu_launches": None}))

@@ -8,10 +8,11 @@ input [1,1,128,128,128,1] -> output [1,1,128,128,128,20]; 1 x N y-pencil over N 
 scaling: the global problem is fixed).  A step = forward + relative-L2 loss + backward + Adam.
 Synthetic fields, random-init weights.
 
-* ``--impl fused``     this framework's sm_100a engine (default)
+* ``--impl fused``     this framework's sm_90a engine (default)
 * ``--impl baseline``  the same algorithm on stock libraries (torch.fft/cuFFT + cuBLAS + NCCL
                        all_to_all/broadcast/reduce): the re-expression BASELINE.md describes
-* ``--impl reference`` the UNMODIFIED reference from baseline/_ref through its own API (its DistributedFNO,
+* ``--impl reference`` the UNMODIFIED reference (oracle/install_reference.sh puts it in oracle/_ref) through its
+                       own API (its DistributedFNO,
                        loss and training loop: fp32, torch.optim.Adam) -- see baseline/reference_arm.py.  DistDL /
                        mpi4py cannot be installed offline, so its imports resolve to baseline/compat, a
                        self-contained torch.distributed (NCCL) stand-in; nothing of dfno_b200 is on that path.
@@ -22,7 +23,12 @@ re-runs the same steps on ONE GPU after the timed regions and the JSON line carr
 
 Timing: W warm-up steps, then K steps between CUDA events bracketed by barrier +
 synchronize; max over ranks.  The per-step working set (>= 1.7 GB of activations per block)
-is far larger than the 126 MB L2, so no explicit flush is needed.
+is far larger than the 50 MB L2 of an H100, so no explicit flush is needed.
+
+``--dump-outputs DIR`` writes, after the timed steps, what the timed step returned and changed in its last
+step: ``loss.npy`` (float64, shape [1]) and ``parameters.npy`` (float32: this rank's flat parameters after the
+update, or a fixed seeded sample of 15 Mi of them when there are more; the whole directory stays below 64 MB).  Inputs and initial weights are
+functions of a fixed seed, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -41,7 +47,9 @@ def parse():
     ap.add_argument("--steps", type=int, default=8)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="fused", choices=["fused", "baseline", "reference"])
-    ap.add_argument("--grid", type=int, default=128)
+    ap.add_argument("--grid", type=int, default=None,
+                    help="global field edge (default 128; 96 for --impl reference on one GPU, where the unfused fp32 "
+                         "reference needs more than the 80 GB of an H100 at 128^3)")
     ap.add_argument("--nt", type=int, default=20)
     ap.add_argument("--width", type=int, default=20)
     ap.add_argument("--modes", type=int, nargs=4, default=[12, 12, 12, 10])
@@ -58,7 +66,30 @@ def parse():
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel eagerly instead of replaying a CUDA graph")
     ap.add_argument("--no-parity", action="store_true",
                     help="skip the N-rank vs 1-rank output / loss comparison that rank 0 runs after the timed regions")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the loss and the updated parameters of the last timed step to DIR/<name>.npy (rank 0)")
+    args = ap.parse_args()
+    if args.grid is None:
+        args.grid = 96 if (args.impl == "reference" and args.gpus == 1) else 128
+    return args
+
+
+DUMP_MAX_PARAMS = 15 * 2 ** 20          # 62.9 MB of float32: with the .npy headers and loss.npy below 64e6 bytes
+
+
+def dump_outputs(out_dir, loss, params):
+    """loss: 0-d tensor; params: list of this rank's parameter tensors after the step."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss.detach())], dtype=np.float64))
+    parts = [torch.view_as_real(p.detach()) if p.is_complex() else p.detach() for p in params]
+    flat = torch.cat([t.reshape(-1).float() for t in parts]) if parts else torch.zeros(0)
+    if flat.numel() > DUMP_MAX_PARAMS:           # fixed seeded positions (with repeats), in memory order
+        g = torch.Generator(device="cpu").manual_seed(4321)
+        idx = torch.randint(flat.numel(), (DUMP_MAX_PARAMS,), generator=g).sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(out_dir, "parameters.npy"), flat.cpu().numpy().astype(np.float32))
 
 
 class ClockSampler:
@@ -120,6 +151,8 @@ class ClockSampler:
 def main():
     args = parse()
     if args.impl == "reference":
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs covers --impl fused / baseline")
         # the unmodified reference through its own API; nothing of dfno_b200 is imported on this path
         sys.path.insert(0, os.path.join(ROOT, "baseline"))
         import reference_arm
@@ -256,6 +289,8 @@ def main():
     total_ms, last_loss = timed(step_device, args.steps)
     launches = (counter.count - c0) if hasattr(counter, "count") else 0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_loss, [p for p in net.parameters() if p.numel() > 0])
     ms_step = total_ms / args.steps
     value = args.batch * 1000.0 / ms_step
     loss_value = float(last_loss)
@@ -310,7 +345,7 @@ def main():
                        "global_batch": args.batch, "seq_len": G * G * G * T,
                        "parallelism": (f"y-pencil 1x{N} (model parallel: field over y, spectral weights over kz)"
                                        if not args.partition else f"P_x = {grid} (model parallel domain decomposition)"),
-                       "l2": "per-step working set (>=0.2 GB/rank/block activations) exceeds the 126 MB L2; no flush needed",
+                       "l2": "per-step working set (>=0.2 GB/rank/block activations) exceeds the 50 MB L2; no flush needed",
                        "step": "forward + DistributedRelativeLpLoss + backward + Adam"},
             "clocks": clocks, "e2e": e2e, "gpu_launches": launches,
             "cuda_graph": bool(tr._graph is not None), "loss": loss_value, "loss_parity": parity,

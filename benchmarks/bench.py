@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Scaling-benchmark kernel: one (input shape, partition, width, modes, nt) point.
 
-Same CLI and per-rank JSON contract as ``/root/reference/benchmarks/bench.py:149-161`` -- keys
+Same CLI and per-rank JSON contract as reference ``benchmarks/bench.py:149-161`` -- keys
 ``dt`` (forward), ``dt_comm`` (time in repartitions/broadcasts), ``dt_comp = dt - dt_comm``
 and, for ``--benchmark-type grad``, ``dt_grad`` (backward from a ones cotangent) -- but
 measured properly: warm-up iterations, a barrier, and CUDA events / synchronised clocks.

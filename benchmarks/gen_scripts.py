@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """Generate weak-scaling run scripts (``{eval,grad}_weak_scaling_{spatial,temporal}_gpu.sh``)
-and a driver ``submit_<system>.sh`` -- the role of ``/root/reference/benchmarks/gen_scripts.py``
+and a driver ``submit_<system>.sh`` -- the role of reference ``benchmarks/gen_scripts.py``
 (Summit/Perlmutter tables at ``:119-161``), re-targeted at one-process-per-GPU ``torchrun``
 launches on NVSwitch boxes:
 
-* ``b200``        : one 8 x B200 box, 64^3 x 32 per GPU, the field grows in x, y and z (grids up to 2x2x2)
-* ``b200-pencil`` : the same box, 1 x N y-pencils at 128 x 16 x 128 x 20 per GPU
+* ``h100``        : one 8 x H100 box, 64^3 x 32 per GPU, the field grows in x, y and z (grids up to 2x2x2)
+* ``h100-pencil`` : the same box, 1 x N y-pencils at 128 x 16 x 128 x 20 per GPU
 * ``local``       : CPU/gloo development runs, N <= 4
 
 "spatial" grows the partitioned extents (and their modes) with the grid at fixed per-GPU size; "temporal"
@@ -17,7 +17,7 @@ from argparse import ArgumentParser
 from pathlib import Path
 
 ap = ArgumentParser()
-ap.add_argument("--system", default="b200", choices=["b200", "b200-pencil", "local"])
+ap.add_argument("--system", default="h100", choices=["h100", "h100-pencil", "local"])
 ap.add_argument("--max-workers", "-mw", type=int, default=-1)
 ap.add_argument("--clean-old", "-co", action="store_true")
 ap.add_argument("--out", type=Path, default=Path(os.path.dirname(os.path.abspath(__file__))))
@@ -25,13 +25,13 @@ args = ap.parse_args()
 
 SYSTEMS = {
     # per-GPU local shape (X, Y, Z, T), per-GPU modes, device, dtype, and the worker grids of the scaling series.
-    # "b200": one 8 x B200 NVSwitch box.  Like the reference's Perlmutter table (gen_scripts.py:141-153: 64^3 x 32 per
+    # "h100": one 8 x H100 NVSwitch box.  Like the reference's Perlmutter table (gen_scripts.py:141-153: 64^3 x 32 per
     # GPU, 4 modes / axis / GPU) the volume grows in every spatial axis -- 1, 2, 4, 8 GPUs = (1,1,1), (1,2,1), (2,2,1),
     # (2,2,2) -- so the 4- and 8-GPU points exercise the general-partition path (folded onto the engine's y-pencil);
-    # "b200-pencil" is the 1 x N y-pencil series (BASELINE config 2's layout) at 128 x 16 x 128 x 20 per GPU.
-    "b200": dict(shape=(64, 64, 64, 32), modes=(4, 4, 4, 4), device="cuda", dtype="bf16",
+    # "h100-pencil" is the 1 x N y-pencil series (BASELINE config 2's layout) at 128 x 16 x 128 x 20 per GPU.
+    "h100": dict(shape=(64, 64, 64, 32), modes=(4, 4, 4, 4), device="cuda", dtype="bf16",
                  grids={1: (1, 1, 1, 1, 1, 1), 2: (1, 1, 1, 2, 1, 1), 4: (1, 1, 2, 2, 1, 1), 8: (1, 1, 2, 2, 2, 1)}),
-    "b200-pencil": dict(shape=(128, 16, 128, 20), modes=(12, 2, 12, 10), device="cuda", dtype="bf16",
+    "h100-pencil": dict(shape=(128, 16, 128, 20), modes=(12, 2, 12, 10), device="cuda", dtype="bf16",
                         grids={n: (1, 1, 1, n, 1, 1) for n in (1, 2, 4, 8)}),
     "local": dict(shape=(16, 8, 16, 8), modes=(4, 2, 4, 4), device="cpu", dtype="fp32",
                   grids={1: (1, 1, 1, 1, 1, 1), 2: (1, 1, 1, 2, 1, 1), 4: (1, 1, 2, 2, 1, 1)}),

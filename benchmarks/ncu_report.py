@@ -1,14 +1,20 @@
 #!/usr/bin/env python
 """Condense an .ncu-rep (read with `ncu -i`) into the numbers the roofline needs.
 
-    ncu_report.py rep.ncu-rep [peaks.json]            last captured launch -> one JSON object
-    ncu_report.py rep.ncu-rep --all [peaks.json]      slowest launch of every distinct kernel -> JSON list
+    ncu_report.py rep.ncu-rep [copy_GBps]             last captured launch -> one JSON object
+    ncu_report.py rep.ncu-rep --all [copy_GBps]       slowest launch of every distinct kernel -> JSON list
+
+copy_GBps: measured device-to-device copy bandwidth (default: the H100 value of dfno_b200.models.fused).
 """
-import csv, io, json, re, subprocess, sys
+import csv, io, json, os, re, subprocess, sys
 args = [a for a in sys.argv[1:] if a != "--all"]
 every = "--all" in sys.argv
 rep = args[0]
-peaks = json.load(open(args[1] if len(args) > 1 else "MEASURED_PEAKS.json"))
+if len(args) > 1:
+    copy_gbs = float(args[1])
+else:
+    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    from dfno_b200.models.fused import H100_COPY_GBS as copy_gbs
 raw = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout
 rows = list(csv.reader(io.StringIO(raw)))
 hdr, units = rows[0], rows[1]
@@ -39,7 +45,7 @@ def condense(vals):
     return {
         "kernel": re.sub(r"\(.*", "", m.get("Kernel Name", ""))[:80], "duration_ms": t * 1e3,
         "dram_read_GB": rd / 1e9, "dram_write_GB": wr / 1e9, "dram_TBps": (rd + wr) / t / 1e12,
-        "frac_of_measured_copy_bw": (rd + wr) / t / 1e9 / peaks["hbm_gbs"],
+        "frac_of_measured_copy_bw": (rd + wr) / t / 1e9 / copy_gbs,
         "dram_throughput_pct_of_peak": f("gpu__dram_throughput.avg.pct_of_peak_sustained_elapsed"),
         "l2_throughput_pct_of_peak": f("lts__throughput.avg.pct_of_peak_sustained_elapsed"),
         "tensor_pipe_active_pct": f("sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active"),

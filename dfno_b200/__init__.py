@@ -1,6 +1,6 @@
-"""dfno_b200 -- a Blackwell-native model-parallel Fourier Neural Operator framework.
+"""dfno_b200 -- a Hopper-native model-parallel Fourier Neural Operator framework.
 
-Public namespace (same names as slimgroup/dfno, ``/root/reference/dfno/__init__.py:1-3``):
+Public namespace (same names as slimgroup/dfno, reference ``dfno/__init__.py:1-3``):
 ``DistributedFNO``, ``DistributedFNONd``, ``DistributedFNOBlock``, ``BroadcastedLinear``,
 ``DistributedRelativeLpLoss``, ``DistributedMSELoss``, ``create_standard_partitions``,
 ``create_root_partition``, ``compute_distribution_info``, ``get_env``, ``alphabet``,

@@ -1,4 +1,4 @@
-// Python bindings (torch extension) for the sm_100a kernels.  The kernels themselves are
+// Python bindings (torch extension) for the sm_90a kernels.  The kernels themselves are
 // torch-free CUDA translation units; this file only unpacks tensors / streams.
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
@@ -76,8 +76,8 @@ void register_ops(pybind11::module& m);    // ops_bindings.cpp
 void register_symm(pybind11::module& m);   // symm_mem.cpp
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "dfno_b200 sm_100a kernels";
-  m.def("dft_gemm", &dft_gemm, "resident-operator GEMM on tcgen05 (see dft_gemm_sm100.cu)",
+  m.doc() = "dfno_b200 sm_90a kernels";
+  m.def("dft_gemm", &dft_gemm, "resident-operator GEMM on wgmma (see dft_gemm_sm90.cu)",
         py::arg("A"), py::arg("M"), py::arg("K"), py::arg("lda"), py::arg("Bmat"), py::arg("N"),
         py::arg("epi"), py::arg("peer_ptrs"), py::arg("add_src") = c10::nullopt, py::arg("ld_add") = 0,
         py::arg("max_ctas") = 0, py::arg("v0") = c10::nullopt, py::arg("v1") = c10::nullopt, py::arg("s0") = 0.0, py::arg("a_f16") = false);

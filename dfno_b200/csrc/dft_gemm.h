@@ -1,4 +1,4 @@
-// Host/device-shared parameter blocks of the resident-operator GEMM (dft_gemm_sm100.cu).
+// Host/device-shared parameter blocks of the resident-operator GEMM (dft_gemm_sm90.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -52,7 +52,7 @@ struct GemmParams {
   int K;         // valid reduction length
   int n_pad;     // operator rows in memory   (multiple of 16, <= 256)
   int k_pad;     // operator row length       (multiple of 64)
-  int a_f16;     // A holds IEEE fp16 instead of bf16 (B stays bf16: mixed-format kind::f16 MMA)
+  int a_f16;     // A holds IEEE fp16 instead of bf16: refused (wgmma has no mixed fp16 x bf16 form)
   EpiParams epi;
 };
 

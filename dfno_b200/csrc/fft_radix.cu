@@ -5,14 +5,14 @@
 // moves the same bytes as an FFT as long as few modes are kept (m <= N/4).  For wide spectra (m > N/4), for
 // un-truncated transforms and for power-of-two axes longer than the GEMM kernel's 256 samples the O(N log N)
 // butterfly network wins; this kernel is that path (reference ops: torch.fft.rfft/fft/ifft/irfft + restrict /
-// zeropad, /root/reference/dfno/dfno.py:252-258,281-285).
+// zeropad, reference dfno/dfno.py:252-258,281-285).
 //
 //   forward   x[line, N] (real or complex) -> X[line, kept modes]     kept = [0,m) (one-sided) or [0,m) u [N-m,N)
 //   inverse   X[line, kept modes] -> x[line, N] (complex, or real via Hermitian completion), scaled 1/N
 //
 // One line = N complex points ping-ponging between two shared-memory arrays; N/4 threads per line; several lines
 // per CTA so that a CTA always has >= 128 threads.  Twiddles come from sincospif (exact argument reduction).
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "kernels.h"
 
 namespace dfno {

@@ -1,0 +1,504 @@
+// head_sm90.cu -- projection head  out = W4 . gelu(W3 h + b3) + b4  (reference linear3 -> gelu -> linear4,
+// dfno.py:348-351; SURVEY.md K17), forward and backward, straight from the engine's CHANNEL-MAJOR activation
+// h[b*C + c][S positions] (no channels-last copy): a tile is 128 consecutive positions of all C channels,
+// dropped into shared memory by TMA as two SWIZZLE_128B boxes of [C rows][64 positions] and used as an
+// MN-major A operand (M = positions, K = channels).  Row C of every tile image is a constant row of ones and
+// column C of the W3 operand holds b3, so the hidden bias rides through the MMA -- and, in the backward, the
+// same ones row turns the tensor core into the reducer for db3.  The 128-channel hidden layer never exists in
+// memory.
+//
+//   forward   MMA   pre[pos, j] = sum_c h[c, pos] W3[j, c] + b3[j]
+//             epi   out[pos]    = b4 + sum_j W4[j] gelu(pre[pos, j])      (packed fp16 GELU, HFMA2 dot)
+//
+//   backward  MMA1  pre (as above)
+//             epi A P[pos, j]   = W4[j] gelu'(pre)  (fp16 tile in smem);  dW4[j] += sum_pos dout gelu(pre)
+//                   hs[c, pos]  = s dout[pos] h[c, pos],  hs[C, pos] = s dout[pos]   (fp16, s = 2^k keeps the
+//                                 loss gradient inside the fp16 range; undone when the sums are flushed)
+//             MMA2  dh0[pos, i]    = sum_j P[pos, j] W3[j, i]          epi B: g[i, pos] = dout[pos] dh0[pos, i]
+//             MMA3  D3[j, i]      += sum_pos P[pos, j] hs[i, pos]      -> dW3 (i < C), db3 (i = C)
+#include "sm90_ptx.cuh"
+#include "kernels.h"
+#include "tma_host.h"
+
+namespace dfno {
+namespace {
+
+constexpr int kHidH = 128;
+
+struct RowMap {                      // position row -> element offset in the public [B,1,X,Y,Z,T] layout
+  int nrl;
+  int R[4];
+  long long SR[4];
+  unsigned long long Rm[4];
+  int Rs[4];
+};
+
+__device__ __forceinline__ long long row_to_offset(const RowMap& e, uint32_t r) {
+  long long off = 0;
+#pragma unroll
+  for (int l = 0; l < 4; ++l) {
+    if (l < e.nrl) {
+      uint32_t d = r;
+      if (l != e.nrl - 1) {
+        const uint32_t q = static_cast<uint32_t>((static_cast<unsigned long long>(r) * e.Rm[l]) >> e.Rs[l]);
+        d = r - q * static_cast<uint32_t>(e.R[l]);
+        r = q;
+      }
+      off += static_cast<long long>(d) * e.SR[l];
+    }
+  }
+  return off;
+}
+
+void fill_magic(RowMap* m) {
+  for (int l = 0; l < 4; ++l) {
+    const unsigned d = static_cast<unsigned>(m->R[l] > 0 ? m->R[l] : 1);
+    int s = 0;
+    while ((1ull << s) < d) ++s;
+    m->Rm[l] = ((1ull << (31 + s)) / d) + 1;
+    m->Rs[l] = 31 + s;
+  }
+}
+
+// ================================================================================ forward
+constexpr int kStagesHF = 6;
+constexpr int kGroupsHF = 2;                    // consumer warpgroups (kStagesHF a multiple of it: see bypass_sm90.cu)
+static_assert(kStagesHF % kGroupsHF == 0, "every ring stage must belong to one consumer warpgroup");
+constexpr int kThreadsHF = 128 * kGroupsHF + 32;
+
+struct HeadFwdParams {
+  int B, C, KR;
+  long long S, tiles_per_b;
+  const float* w4b4;          // [128 weights, 1 bias]
+  float* out;
+  RowMap map;
+};
+
+__global__ void __launch_bounds__(kThreadsHF, 1)
+head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
+                const HeadFwdParams p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* s_w3 = smem;                                    // [128 hid][64] K-major, column C = b3
+  uint8_t* s_a = smem + 16384;                             // stages x 2 halves x [KR rows][64 pos]
+  const uint32_t half_bytes = static_cast<uint32_t>(p.KR) * 128;
+  const uint32_t stage_bytes = 2 * half_bytes;
+  float* s_scratch = reinterpret_cast<float*>(s_a + kStagesHF * stage_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_scratch + 4 * kGroupsHF * kRowScratchFloats);
+  uint64_t* full = bars;              // [6]
+  uint64_t* empty = bars + 6;         // [6]
+  uint64_t* wfull = bars + 12;
+  uint32_t* s_w4 = reinterpret_cast<uint32_t*>(bars + 14);   // [64] fp16x2 pairs of W4 (16-byte aligned)
+  float* s_b4 = reinterpret_cast<float*>(s_w4 + 64);
+
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const long long num_tiles = p.tiles_per_b * p.B;
+
+  for (uint32_t i = threadIdx.x; i < kStagesHF * stage_bytes / 16; i += blockDim.x)
+    reinterpret_cast<uint4*>(s_a)[i] = make_uint4(0, 0, 0, 0);
+  __syncthreads();
+  for (uint32_t i = threadIdx.x; i < kStagesHF * 2 * 16; i += blockDim.x) {      // the ones row (row C) of every half
+    const uint32_t hb = i >> 4, ch = i & 15;
+    reinterpret_cast<uint2*>(s_a + hb * half_bytes + p.C * 128)[ch] = make_uint2(0x3F803F80u, 0x3F803F80u);
+  }
+  for (int i = threadIdx.x; i < 64; i += blockDim.x)
+    s_w4[i] = h2_bits(h2_from_f32(p.w4b4[2 * i], p.w4b4[2 * i + 1]));
+  if (threadIdx.x == 0) s_b4[0] = p.w4b4[kHidH];
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmH); tma_prefetch_desc(&tmW3);
+    for (int s = 0; s < kStagesHF; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+    mbar_init(wfull, 1);
+    fence_barrier_init();
+  }
+  fence_proxy_async_smem();
+  __syncthreads();
+
+  if (warp == 4 * kGroupsHF) {
+    if (lane == 0) {
+      mbar_arrive_expect_tx(wfull, 16384);
+      tma_load_2d(s_w3, &tmW3, wfull, 0, 0);
+      uint32_t s = 0, ph = 0;
+      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int b = static_cast<int>(tile / p.tiles_per_b);
+        const int p0 = static_cast<int>((tile % p.tiles_per_b) * 128);
+        mbar_wait(&empty[s], ph ^ 1);
+        mbar_arrive_expect_tx(&full[s], 2u * p.C * 128);
+        uint8_t* st = s_a + s * stage_bytes;
+        tma_load_2d(st, &tmH, &full[s], p0, b * p.C);
+        tma_load_2d(st + half_bytes, &tmH, &full[s], p0 + 64, b * p.C);
+        if (++s == kStagesHF) { s = 0; ph ^= 1; }
+      }
+    }
+    return;
+  }
+  const int q = warp & 3, g = warp >> 2;
+  const int m = wg_row128(q, lane);
+  float* scratch = s_scratch + warp * kRowScratchFloats;
+  const float b4 = s_b4[0];
+  const int ksteps = p.KR >> 4;
+  const uint32_t w_addr = smem_u32(s_w3);
+  mbar_wait(wfull, 0);
+  float acc[128];
+  long long n = 0;
+  for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
+    if (n % kGroupsHF != g) continue;
+    const uint32_t s = static_cast<uint32_t>(n % kStagesHF);
+    const int b = static_cast<int>(tile / p.tiles_per_b);
+    const long long pos = (tile % p.tiles_per_b) * 128 + m;
+    mbar_wait(&full[s], (n / kStagesHF) & 1);
+    // pre[pos, j] = sum_c h[c, pos] W3aug[j, c]: A MN-major (positions contiguous, 64-position halves half_bytes apart)
+    const uint32_t abase = smem_u32(s_a + s * stage_bytes);
+    wgmma_fence();
+    for (int ks = 0; ks < ksteps; ++ks)
+      wg_mma128<false, 1, 0>(acc, kHidH, gdesc_mn128(abase + ks * 2048, half_bytes, 1024), half_bytes,
+                             gdesc_k128(w_addr + ks * 32), ks > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(acc);
+    if (q == 0 && lane == 0) mbar_arrive(&empty[s]);
+    float out = b4;
+#pragma unroll
+    for (int ch = 0; ch < 8; ++ch) {
+      uint32_t v[16];
+      wg_row16<2>(acc, ch * 16, scratch, v);
+      const uint4 wa = reinterpret_cast<const uint4*>(s_w4)[2 * ch], wb = reinterpret_cast<const uint4*>(s_w4)[2 * ch + 1];
+      const uint32_t w[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w};
+      __half2 part = __float2half2_rn(0.f);
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        part = __hfma2(gelu_h2(h2_from_f32(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]))),
+                       h2_of_bits(w[i]), part);
+      const float2 f = __half22float2(part);
+      out += f.x + f.y;
+    }
+    if (pos < p.S) p.out[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] = out;
+  }
+}
+
+// ================================================================================ backward
+constexpr int kMaxStagesHB = 6;                 // h tiles are small: deep prefetch keeps TMA latency off the consumers
+constexpr int kGroupsHB = 2;                    // consumer warpgroups (stages a multiple of it: see bypass_sm90.cu)
+constexpr int kThreadsHB = 128 * kGroupsHB + 32;
+
+struct HeadBwdParams {
+  int B, C, KR, stages;
+  long long S, tiles_per_b;
+  const float* dout;          // fp32, public layout
+  const float* amax;          // max |dout| (device scalar)
+  const float* W4;
+  __nv_bfloat16* g;           // [B*C, S]
+  float* gW3; float* gb3; float* gW4; float* gb4;
+  RowMap map;
+};
+
+// Per tile of 128 positions, one consumer warpgroup runs the backward of the file header; MMA1 in two
+// 64-column halves so that the D3 accumulator fits next to it.
+// KR: channels + the ones row, padded to 16 (the N of MMA2 / MMA3 and the accumulator width)
+template <int KR>
+__global__ void __launch_bounds__(kThreadsHB, 1)
+head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
+                 const __grid_constant__ CUtensorMap tmW3T, const HeadBwdParams p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const uint32_t half_bytes = static_cast<uint32_t>(KR) * 128;
+  const uint32_t tile_bytes = 2 * half_bytes;
+  uint8_t* s_w3 = smem;                                   // 16 KB
+  uint8_t* s_w3t = s_w3 + 16384;                          // 2 k-blocks x [KR c rows][64 hid] fp16
+  uint8_t* s_p = s_w3t + tile_bytes;                      // per warpgroup: 2 x [128 pos][64 hid] fp16
+  uint8_t* s_a = s_p + kGroupsHB * 32768;                 // stages x h tile
+  uint8_t* s_hs = s_a + p.stages * tile_bytes;            // per warpgroup: scaled fp16 copy of the h tile
+  float* s_scratch = reinterpret_cast<float*>(s_hs + kGroupsHB * tile_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_scratch + 4 * kGroupsHB * kRowScratchFloats);
+  uint64_t* a_full = bars;            // [8]
+  uint64_t* a_empty = bars + 8;       // [8]
+  uint64_t* w_full = bars + 16;
+  float* s_gb4 = reinterpret_cast<float*>(bars + 18);
+  uint32_t* s_w4h = reinterpret_cast<uint32_t*>(bars + 20);   // [64] fp16x2 pairs of W4 (16-byte aligned)
+  float* s_gw4 = reinterpret_cast<float*>(s_w4h + 64);       // [128] CTA partial sums of dW4
+
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const long long num_tiles = p.tiles_per_b * p.B;
+
+  for (uint32_t i = threadIdx.x; i < p.stages * tile_bytes / 16; i += blockDim.x)
+    reinterpret_cast<uint4*>(s_a)[i] = make_uint4(0, 0, 0, 0);
+  for (uint32_t i = threadIdx.x; i < kGroupsHB * tile_bytes / 16; i += blockDim.x)
+    reinterpret_cast<uint4*>(s_hs)[i] = make_uint4(0, 0, 0, 0);
+  __syncthreads();
+  for (uint32_t i = threadIdx.x; i < static_cast<uint32_t>(p.stages) * 2 * 16; i += blockDim.x) {
+    const uint32_t hb = i >> 4, ch = i & 15;
+    reinterpret_cast<uint2*>(s_a + hb * half_bytes + p.C * 128)[ch] = make_uint2(0x3F803F80u, 0x3F803F80u);
+  }
+  if (threadIdx.x == 0) s_gb4[0] = 0.f;
+  for (int i = threadIdx.x; i < 64; i += blockDim.x) s_w4h[i] = h2_bits(h2_from_f32(p.W4[2 * i], p.W4[2 * i + 1]));
+  for (int i = threadIdx.x; i < kHidH; i += blockDim.x) s_gw4[i] = 0.f;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmH); tma_prefetch_desc(&tmW3); tma_prefetch_desc(&tmW3T);
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
+    mbar_init(w_full, 1);
+    fence_barrier_init();
+  }
+  fence_proxy_async_smem();
+  __syncthreads();
+  const float amax = *p.amax;
+  const float scale = amax > 0.f ? exp2f(-ceilf(log2f(amax))) : 1.0f;      // |scale * dout| <= 1
+
+  if (warp == 4 * kGroupsHB) {
+    if (lane == 0) {
+      mbar_arrive_expect_tx(w_full, 16384 + tile_bytes);
+      tma_load_2d(s_w3, &tmW3, w_full, 0, 0);
+      tma_load_2d(s_w3t, &tmW3T, w_full, 0, 0);
+      tma_load_2d(s_w3t + half_bytes, &tmW3T, w_full, 64, 0);
+      uint32_t s = 0, ph = 0;
+      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int b = static_cast<int>(tile / p.tiles_per_b);
+        const int p0 = static_cast<int>((tile % p.tiles_per_b) * 128);
+        mbar_wait(&a_empty[s], ph ^ 1);
+        mbar_arrive_expect_tx(&a_full[s], 2u * p.C * 128);
+        uint8_t* st = s_a + s * tile_bytes;
+        tma_load_2d(st, &tmH, &a_full[s], p0, b * p.C);
+        tma_load_2d(st + half_bytes, &tmH, &a_full[s], p0 + 64, b * p.C);
+        if (++s == static_cast<uint32_t>(p.stages)) { s = 0; ph ^= 1; }
+      }
+    }
+    return;
+  }
+
+  const int q = warp & 3, g = warp >> 2;
+  const int m = wg_row128(q, lane);                  // position inside the tile
+  float* scratch = s_scratch + warp * kRowScratchFloats;
+  const uint32_t barid = 1 + g;
+  const int k1steps = KR >> 4;
+  uint8_t* pbuf = s_p + g * 32768;
+  uint8_t* hsbuf = s_hs + g * tile_bytes;
+  const uint32_t w3_addr = smem_u32(s_w3), w3t_addr = smem_u32(s_w3t);
+  const uint32_t p_addr = smem_u32(pbuf), hs_addr = smem_u32(hsbuf);
+  float acc_gb4 = 0.f;
+  float d3[KR];                                      // [hid, c] over this warpgroup's tiles: 128 x KR
+  long long n = 0, mine = 0;
+  mbar_wait(w_full, 0);
+  for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
+    if (n % kGroupsHB != g) continue;
+    const uint32_t s = static_cast<uint32_t>(n % p.stages);
+    const int b = static_cast<int>(tile / p.tiles_per_b);
+    const long long pos = (tile % p.tiles_per_b) * 128 + m;
+    const float dout = pos < p.S ? p.dout[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] : 0.f;
+    acc_gb4 += dout;
+    mbar_wait(&a_full[s], (n / p.stages) & 1);
+    const uint32_t abase = smem_u32(s_a + s * tile_bytes);
+    uint8_t* prow = pbuf + m * 128;
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {                         // hidden units [64 hh, 64 hh + 64)
+      float acc[64];
+      wgmma_fence();
+      for (int ks = 0; ks < k1steps; ++ks)
+        wg_mma128<false, 1, 0>(acc, 64, gdesc_mn128(abase + ks * 2048, half_bytes, 1024), half_bytes,
+                               gdesc_k128(w3_addr + hh * 8192 + ks * 32), ks > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc);
+#pragma unroll
+      for (int ch = 0; ch < 4; ++ch) {                       // 16 hidden units per chunk
+        uint32_t v[16];
+        wg_row16<2>(acc, ch * 16, scratch, v);
+        const uint4 w4 = reinterpret_cast<const uint4*>(s_w4h + 32 * hh + 8 * ch)[0];
+        const uint4 w4b = reinterpret_cast<const uint4*>(s_w4h + 32 * hh + 8 * ch)[1];
+        const uint32_t ww[8] = {w4.x, w4.y, w4.z, w4.w, w4b.x, w4b.y, w4b.z, w4b.w};
+        uint32_t pw[8];
+        float wsum[16];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const GeluH2 vg = gelu_vg_h2(h2_from_f32(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1])));
+          pw[i] = h2_bits(__hmul2(vg.grad, h2_of_bits(ww[i])));
+          const float2 a = __half22float2(vg.value);
+          wsum[2 * i] = dout * a.x;
+          wsum[2 * i + 1] = dout * a.y;
+        }
+        const uint32_t chunk = 2 * ch;                       // 16-byte chunks of this row in the 64-wide hid block
+        uint8_t* blk = prow + hh * 16384;
+        *reinterpret_cast<uint4*>(blk + ((chunk ^ (m & 7)) << 4)) = make_uint4(pw[0], pw[1], pw[2], pw[3]);
+        *reinterpret_cast<uint4*>(blk + (((chunk + 1) ^ (m & 7)) << 4)) = make_uint4(pw[4], pw[5], pw[6], pw[7]);
+        const float sw = warp_transpose_reduce16(wsum, lane);
+        if (lane < 16) atomicAdd(&s_gw4[64 * hh + 16 * ch + lane], sw);
+      }
+    }
+    {
+      // ---- hs: scaled fp16 copy of this position's column; row C = the scaled gradient itself
+      const float ds = dout * scale;
+      const uint32_t colo = (m >> 6) * half_bytes + ((m & 7) << 1);
+      const uint32_t ch = (m & 63) >> 3;
+      const uint8_t* src = s_a + s * tile_bytes;
+#pragma unroll
+      for (int c = 0; c < 32; ++c) {
+        if (c < p.C) {
+          const uint32_t off = colo + c * 128 + ((ch ^ (c & 7)) << 4);
+          const uint16_t hv = *reinterpret_cast<const uint16_t*>(src + off);
+          *reinterpret_cast<__half*>(hsbuf + off) = __float2half_rn(__uint_as_float(static_cast<uint32_t>(hv) << 16) * ds);
+        }
+      }
+      *reinterpret_cast<__half*>(hsbuf + colo + p.C * 128 + ((ch ^ (p.C & 7)) << 4)) = __float2half_rn(ds);
+    }
+    fence_proxy_async_smem();
+    asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
+    float acc2[KR];                                          // dh0 [pos, c]: 128 x KR
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {                         // K = hid
+      const uint32_t kb = ks >> 2, kk = ks & 3;
+      wg_mma128<true, 0, 0>(acc2, KR, gdesc_k128(p_addr + kb * 16384 + kk * 32), 8192,
+                            gdesc_k128(w3t_addr + kb * half_bytes + kk * 32), ks > 0 ? 1u : 0u);
+    }
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {                         // K = positions; A = P read MN-major (hid contiguous)
+      const uint32_t kb = ks >> 2, kk = ks & 3;
+      wg_mma128<true, 1, 0>(d3, KR, gdesc_mn128(p_addr + ks * 2048, 16384, 1024), 16384,
+                            gdesc_k128(hs_addr + kb * half_bytes + kk * 32), (mine > 0 || ks > 0) ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(acc2);
+    acc_fence(d3);
+    ++mine;
+    if (q == 0 && lane == 0) mbar_arrive(&a_empty[s]);
+    // ---- epi B: g[c, pos] = dout * dh0[pos, c]
+#pragma unroll
+    for (int cb = 0; cb < KR / 16; ++cb) {
+      {
+        uint32_t v[16];
+        wg_row16<2>(acc2, cb * 16, scratch, v);
+        if (pos < p.S) {
+          __nv_bfloat16* gp = p.g + (static_cast<long long>(b) * p.C + 16 * cb) * p.S + pos;
+#pragma unroll
+          for (int i = 0; i < 16; ++i)
+            if (16 * cb + i < p.C) gp[static_cast<long long>(i) * p.S] = __float2bfloat16(dout * __uint_as_float(v[i]));
+        }
+      }
+    }
+  }
+  // ---- per-CTA flush of the weight gradients
+  acc_gb4 += __shfl_xor_sync(0xffffffffu, acc_gb4, 16);
+  acc_gb4 += __shfl_xor_sync(0xffffffffu, acc_gb4, 8);
+  acc_gb4 += __shfl_xor_sync(0xffffffffu, acc_gb4, 4);
+  acc_gb4 += __shfl_xor_sync(0xffffffffu, acc_gb4, 2);
+  acc_gb4 += __shfl_xor_sync(0xffffffffu, acc_gb4, 1);
+  if (lane == 0) atomicAdd(s_gb4, acc_gb4);
+  if (mine > 0) {
+    // fragment of the 128 x KR accumulator: register (KR/2)h + 4j + e holds hidden unit 64h + 16q + lane/4 + 8(e/2),
+    // column 8j + 2(lane%4) + e%2
+    const float inv = 1.0f / scale;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < KR / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int hid = 64 * h + 16 * q + (lane >> 2) + 8 * (e >> 1), c = 8 * j + 2 * (lane & 3) + (e & 1);
+          const float v = d3[(KR / 2) * h + 4 * j + e] * inv;
+          {
+            if (c < p.C) atomicAdd(p.gW3 + hid * p.C + c, v);
+            else if (c == p.C) atomicAdd(p.gb3 + hid, v);
+          }
+        }
+  }
+  asm volatile("bar.sync 3, %0;" ::"n"(128 * kGroupsHB) : "memory");
+  if (num_tiles > blockIdx.x && threadIdx.x < kHidH) {
+    atomicAdd(p.gW4 + threadIdx.x, s_gw4[threadIdx.x]);
+    if (threadIdx.x == 0) atomicAdd(p.gb4, s_gb4[0]);
+  }
+}
+
+__global__ void absmax_kernel(const float* __restrict__ x, long long n, unsigned* __restrict__ out) {
+  float mx = 0.f;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i * 4 < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    if (i * 4 + 3 < n) {
+      const float4 v = reinterpret_cast<const float4*>(x)[i];
+      mx = fmaxf(mx, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+    } else {
+      for (long long k = i * 4; k < n; ++k) mx = fmaxf(mx, fabsf(x[k]));
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0 && mx > 0.f) atomicMax(out, __float_as_uint(mx));   // non-negative floats order like uints
+}
+
+int set_rowmap(RowMap* mp, int nrl, const int* R, const long long* SR) {
+  if (nrl < 1 || nrl > 4) return -1;
+  mp->nrl = nrl;
+  for (int i = 0; i < 4; ++i) { mp->R[i] = i < nrl ? R[i] : 1; mp->SR[i] = i < nrl ? SR[i] : 0; }
+  fill_magic(mp);
+  return 0;
+}
+
+}  // namespace
+
+// h: bf16 [B*C, S] channel-major; W3aug: bf16 [128, 64] with column C = b3; w4b4: fp32 [129]; out: fp32, addressed
+// through the row digits (row = b*S + position).
+const char* head_fwd(const void* h, const void* W3aug, const float* w4b4, float* out, int B, int C, long long S,
+                     int nrl, const int* R, const long long* SR, int num_sms, cudaStream_t stream) {
+  if (C < 1 || C > 47) return "head_fwd: 1 <= C <= 47";
+  if (S % 8 || S > (1ll << 31) - 256 || static_cast<long long>(B) * S > (1ll << 31) - 256) return "head_fwd: bad slab size";
+  HeadFwdParams p{};
+  p.B = B; p.C = C; p.KR = (C + 1 + 15) / 16 * 16; p.S = S; p.tiles_per_b = (S + 127) / 128;
+  p.w4b4 = w4b4; p.out = out;
+  if (set_rowmap(&p.map, nrl, R, SR)) return "head_fwd: 1..4 row digits";
+  CUtensorMap tmH, tmW3;
+  if (make_map_2d(&tmH, h, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (h) failed";
+  if (make_map_2d(&tmW3, W3aug, 64, 128, 64, 64, 128)) return "tensor map (W3) failed";
+  static bool attr = false;
+  if (!attr) {
+    if (cudaFuncSetAttribute(head_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+      return "cudaFuncSetAttribute failed";
+    attr = true;
+  }
+  const uint32_t smem_bytes = 16384 + kStagesHF * 2 * p.KR * 128 + 4 * kGroupsHF * kRowScratchFloats * 4 + 2048 + 1024;
+  const long long tiles = p.tiles_per_b * B;
+  const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
+  head_fwd_kernel<<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
+// W3T16: fp16 [KR, 128] (rows = input channel, zero padded); dout: fp32 public layout; amax_ws: one uint of scratch
+// (receives max |dout|); g: bf16 [B*C, S]; gradients are accumulated with atomics.
+const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const float* W4, const float* dout,
+                      long long n_dout, unsigned* amax_ws, void* g, float* gW3, float* gb3, float* gW4, float* gb4,
+                      int B, int C, long long S, int nrl, const int* R, const long long* SR, int num_sms,
+                      cudaStream_t stream) {
+  if (C < 1 || C > 32) return "head_bwd: 1 <= C <= 32";
+  if (S % 8 || S > (1ll << 31) - 256 || static_cast<long long>(B) * S > (1ll << 31) - 256) return "head_bwd: bad slab size";
+  HeadBwdParams p{};
+  p.B = B; p.C = C; p.KR = (C + 1 + 15) / 16 * 16; p.S = S; p.tiles_per_b = (S + 127) / 128;
+  p.dout = dout; p.amax = reinterpret_cast<const float*>(amax_ws); p.W4 = W4;
+  p.g = static_cast<__nv_bfloat16*>(g); p.gW3 = gW3; p.gb3 = gb3; p.gW4 = gW4; p.gb4 = gb4;
+  if (set_rowmap(&p.map, nrl, R, SR)) return "head_bwd: 1..4 row digits";
+  CUtensorMap tmH, tmW3, tmW3T;
+  if (make_map_2d(&tmH, h, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (h) failed";
+  if (make_map_2d(&tmW3, W3aug, 64, 128, 64, 64, 128)) return "tensor map (W3) failed";
+  if (make_map_2d(&tmW3T, W3T16, 128, p.KR, 128, 64, p.KR)) return "tensor map (W3T) failed";
+  static bool attr[3] = {false, false, false};
+  const int kr_i = p.KR / 16 - 1;
+  const void* fn = kr_i == 0 ? reinterpret_cast<const void*>(head_bwd2_kernel<16>)
+                 : kr_i == 1 ? reinterpret_cast<const void*>(head_bwd2_kernel<32>)
+                             : reinterpret_cast<const void*>(head_bwd2_kernel<48>);
+  if (!attr[kr_i]) {
+    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+      return "cudaFuncSetAttribute failed";
+    attr[kr_i] = true;
+  }
+  if (cudaMemsetAsync(amax_ws, 0, 4, stream) != cudaSuccess) return "head_bwd: memset failed";
+  absmax_kernel<<<num_sms * 4, 256, 0, stream>>>(dout, n_dout, amax_ws);
+  const uint32_t tile_bytes = 2u * p.KR * 128;
+  const uint32_t fixed = 16384 + tile_bytes + kGroupsHB * (32768 + tile_bytes) + 4 * kGroupsHB * kRowScratchFloats * 4 +
+                         2048 + 1024;
+  p.stages = kMaxStagesHB;
+  while (p.stages > kGroupsHB && fixed + p.stages * tile_bytes > 227 * 1024) p.stages -= kGroupsHB;
+  const uint32_t smem_bytes = fixed + p.stages * tile_bytes;
+  const long long tiles = p.tiles_per_b * B;
+  const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
+  if (kr_i == 0) head_bwd2_kernel<16><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, p);
+  else if (kr_i == 1) head_bwd2_kernel<32><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, p);
+  else head_bwd2_kernel<48><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, p);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
+}  // namespace dfno

@@ -29,7 +29,7 @@ const char* bypass_gelu_fwd(const void* h, void* spec_pre, const float* W, void*
 const char* bypass_gelu_bwd(const void* dout, const void* dout_cl, int cl_pitch, const void* pre, const float* W,
                             void* dpre, void* dhb, int B, int C, long long S, int num_sms, cudaStream_t s);
 
-// tcgen05 versions (bypass_sm100.cu): TMA in/out, channel mixing on the tensor core, dW accumulated in TMEM.
+// wgmma versions (bypass_sm90.cu): TMA in/out, channel mixing on the tensor core, dW accumulated in registers.
 // Wpad / WTpad: bf16 [32, 64] zero-padded W[o, i] / W^T[i, o].  Need C <= 32 and S % 128 == 0.
 const char* bypass_fwd_tc(const void* h, void* spec_pre, const void* Wpad, void* out, void* out_cl, int cl_pitch,
                           int B, int C, long long S, int save_pre, int num_sms, cudaStream_t stream);
@@ -66,7 +66,7 @@ const char* p2p_alltoall(const void* send, const long long* send_off, void* cons
 const char* kreduce_gemm(const void* A, long long lda, int Ma, const void* Bm, long long ldb, int Nb, long long K,
                          float* D, long long ldd, int num_sms, cudaStream_t s);
 
-// backward of the projection head (head_bwd_sm100.cu).  dout is read at the mixed-radix address
+// backward of the projection head (head_bwd_sm90.cu).  dout is read at the mixed-radix address
 // of each row (public [B,1,X,Y,Z,T] layout); gradients are accumulated with atomics.
 const char* head_bwd(const void* hcl, long long npos, int C, int CP, const void* W3pad, const void* W3Tpad,
                      const float* b3, const float* W4, const float* dout, int nrl, const int* R, const long long* SR,
@@ -77,7 +77,7 @@ const char* fft_radix(const void* x, void* y, int bf16, int N, long long lines, 
                       int one_sided, int m, int num_sms, cudaStream_t s);
 
 // First two stages of a Fourier layer (truncated z-DFT then t-DFT) + the pencil transpose R2 in one kernel: see
-// spectral_in_sm100.cu.  dst_ptrs[j] (+ dst_off elements): rank j's S1 / S1s, viewed [B*C, kzl, mt, X, Yl*2] with
+// spectral_in_sm90.cu.  dst_ptrs[j] (+ dst_off elements): rank j's S1 / S1s, viewed [B*C, kzl, mt, X, Yl*2] with
 // element strides dstr = {x, kt, kz, bc}.
 const char* spectral_in(const void* h, const void* op1, int n1_pad, int k1_pad, const void* op2, int n2_pad, int k2_pad,
                         const long long* dst_ptrs, int P, long long dst_off, const long long* dstr, int BC, int X,
@@ -91,8 +91,8 @@ const char* sq_partials(const float* yh, const float* y, float* part, long long 
 const char* scaled_diff(const float* yh, const float* y, const float* scale, float* grad, long long n_per_b, int B,
                         int scale_per_b, int num_sms, cudaStream_t s);
 
-// ---- round-2 fused pointwise path (spectral_out_sm100.cu, dpre_dw_sm100.cu, head_sm100.cu) ----
-// Last stage of a Fourier layer + bypass conv (+ GELU): see spectral_out_sm100.cu.  U: bf16 [B*C, L, K1];
+// ---- round-2 fused pointwise path (spectral_out_sm90.cu, dpre_dw_sm90.cu, head_sm90.cu) ----
+// Last stage of a Fourier layer + bypass conv (+ GELU): see spectral_out_sm90.cu.  U: bf16 [B*C, L, K1];
 // h / pre / out: bf16 [B*C, L, Z]; Bop: padded operator bf16 [n_pad, k_pad]; W: fp32 [C, C].
 const char* spectral_out(const void* U, const void* h, const void* Bop, int n_pad, int k_pad, const float* W,
                          int transpose_w, void* pre, void* out, int B, int C, long long L, int Z, int K1, int gelu,
@@ -100,7 +100,7 @@ const char* spectral_out(const void* U, const void* h, const void* Bop, int n_pa
 // dpre = g * gelu'(pre) (in place over pre); dW += dpre . h^T
 const char* dpre_dw(const void* g, void* pre_dpre, const void* h, float* dW, int B, int C, long long L, int Z,
                     int num_sms, cudaStream_t stream);
-// projection head on the channel-major activation (head_sm100.cu)
+// projection head on the channel-major activation (head_sm90.cu)
 const char* head_fwd(const void* h, const void* W3aug, const float* w4b4, float* out, int B, int C, long long S,
                      int nrl, const int* R, const long long* SR, int num_sms, cudaStream_t stream);
 const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const float* W4, const float* dout,

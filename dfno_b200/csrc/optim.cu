@@ -2,7 +2,7 @@
 // All parameters of the fused model (pointwise weights and every spectral shard) live in one
 // contiguous allocation, so one vectorised launch updates the whole model
 // (reference: torch.optim.Adam, train_two_phase.py:82, experiment_navier_stokes.py:120).
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "kernels.h"
 
 namespace dfno {

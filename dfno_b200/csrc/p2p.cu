@@ -16,7 +16,7 @@
 //                        the gradient reduction of the replicated pointwise weights -- the
 //                        Broadcast/SumReduce pair of the reference's BroadcastedLinear
 //                        (SURVEY.md K1, K18) collapses to one such call per optimizer step.
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "kernels.h"
 
 namespace dfno {

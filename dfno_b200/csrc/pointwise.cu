@@ -1,7 +1,7 @@
-// pointwise.cu -- channel/time mixing kernels around the Fourier layers (sm_100a, CUDA cores).
+// pointwise.cu -- channel/time mixing kernels around the Fourier layers (sm_90a, CUDA cores).
 //
 // Internal activation layout of the fused engine: h[bc = b*C + c][x][y_local][t][z], bf16,
-// z contiguous (so that every DFT stage is a K-major GEMM, see dft_gemm_sm100.cu).  The
+// z contiguous (so that every DFT stage is a K-major GEMM, see dft_gemm_sm90.cu).  The
 // public tensors keep the reference layout [B, C, X, Y, Z, T] (t contiguous); the lift and
 // the projection head are where the two layouts meet, so no transpose pass ever runs.
 //
@@ -11,7 +11,7 @@
 //   bypass_gelu_fwd : pre = spec + W ._c h ; out = gelu(pre)         (K2 + K14, dfno.py:244,291)
 //   bypass_gelu_bwd : dpre = dout * gelu'(pre) ; dhb = W^T ._c dpre  (weight grad: kreduce GEMM)
 //   to_channels_last / from_channels_last : layout bridges for the projection head
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "kernels.h"
 
 namespace dfno {
@@ -35,7 +35,7 @@ __device__ __forceinline__ float ldf<__nv_bfloat16>(const __nv_bfloat16* p) { re
 // lift
 // ------------------------------------------------------------------------------------------
 // One thread owns 8 consecutive z of one (b, x, y) -- a 16-byte bf16 vector of every output row it produces,
-// so a warp writes whole 256-byte z-lines -- and walks t and c.  Both GELUs run in packed fp16 (sm100_ptx.cuh):
+// so a warp writes whole 256-byte z-lines -- and walks t and c.  Both GELUs run in packed fp16 (sm90_ptx.cuh):
 // the outer one is evaluated B*C*X*Y*Z*T times per step.  The few input values a thread needs stay in
 // registers when Tin == 1 (the benchmark / two-phase case) and are re-read through L1 otherwise (Cin <= 4, Tin <= 64).
 constexpr int kLiftMaxTin = 64;
@@ -136,8 +136,8 @@ lift_fwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
 
 // dW1[T][Tin], db1[T], dW2[C][Cin], db2[C] accumulated with atomics into fp32 buffers.  Four adjacent lanes share
 // one item (8 consecutive z of one (b, x, y)) and split the C channels between them: a thread keeps C/4 channel
-// sums in registers over the whole grid-stride loop (with all C channels per thread the kernel needed 241
-// registers and ran at 12 % occupancy, 0.21 of copy bandwidth: profiles/r2_ncu_kernels.json), the input-gradient
+// sums in registers over the whole grid-stride loop (with all C channels per thread the kernel needs about twice
+// the registers and far lower occupancy), the input-gradient
 // partials of the four quarters meet in two shuffles per value, and time-indexed sums are warp-reduced once per
 // t.  The loss gradient can be far below the fp16 range, so everything it multiplies is fp32; only the GELU'
 // evaluations are packed fp16.

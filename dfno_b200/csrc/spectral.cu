@@ -7,7 +7,7 @@
 // once: the op is bound by streaming the fp32 weights (113-442 MB per block), i.e. a
 // bandwidth problem for plain FMA units with fully coalesced 8-byte loads, not a tensor-core
 // problem.  The backward makes ONE pass over R and produces both dX and dR.
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "kernels.h"
 
 namespace dfno {

@@ -2,7 +2,7 @@
 //
 // Every rank cudaMalloc's a buffer, exports a CUDA IPC handle, and maps the handles of all
 // other ranks of the box (handles travel through the torch.distributed control plane).  The
-// result is a table of device pointers -- one per rank -- that sm_100a kernels dereference
+// result is a table of device pointers -- one per rank -- that sm_90a kernels dereference
 // directly: stores/loads to a peer pointer are routed over NVLink 5 / NVSwitch by the
 // hardware.  This replaces the MPI communicator the reference reaches through DistDL
 // (SURVEY.md §5.8) for everything on the hot path.

@@ -4,7 +4,7 @@
   (anything with ``read(sample, name, slices) -> ndarray``), with global min/max
   normalisation by MIN/MAX all-reduce over the partition and an optional per-rank on-disk
   cache ``{filename}_{sample:04d}_{rank:04d}.npz``.  This is the role of
-  ``/root/reference/training/two_phase/sleipner_dataset.py:12-121`` (Azure-blob Zarr store,
+  reference ``training/two_phase/sleipner_dataset.py:12-121`` (Azure-blob Zarr store,
   HDF5 cache, raw MPI allreduce), generalised: the reference slices only the y axis
   (``:51-55``); here the slab follows the rank's ``P_x`` index on every spatial axis.
 * stores: :class:`SyntheticTwoPhaseStore` (procedural CO2-plume-like fields: no network or

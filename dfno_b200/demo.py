@@ -1,6 +1,6 @@
 """Smoke demo: ``python -m dfno_b200.demo`` (or under torchrun with 4 ranks).
 
-Counterpart of the ``__main__`` block of ``/root/reference/dfno/dfno.py:355-389``: build a
+Counterpart of the ``__main__`` block of reference ``dfno/dfno.py:355-389``: build a
 64^3 network with 30 output steps, run a few forward/backward passes and print per-rank
 times -- device-timed instead of bare host clocks."""
 import time

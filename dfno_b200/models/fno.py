@@ -1,12 +1,12 @@
 """Model-parallel Fourier Neural Operator -- portable (torch.fft / torch.distributed) backend.
 
 This backend defines the *semantics* of the framework: any device, fp32/fp64 (bf16 is
-up-cast inside the transforms), any Cartesian partition, gloo or NCCL.  On B200 the fused
-sm_100a engine (:mod:`dfno_b200.models.fused`) computes the same function; run over NCCL,
+up-cast inside the transforms), any Cartesian partition, gloo or NCCL.  On H100 the fused
+sm_90a engine (:mod:`dfno_b200.models.fused`) computes the same function; run over NCCL,
 this backend is also the measured baseline (``bench.py --impl baseline``).
 
 Mathematical specification of one block (SURVEY.md §3.1; reference
-``/root/reference/dfno/dfno.py:241-291``)::
+reference ``dfno/dfno.py:241-291``)::
 
     y0  = W_lin ._c x                                          (no bias)
     X^  = Trunc( FFT_{axes 1..n-1}( RFFT_{axis n}(x) ) )       keep [0,m) u [N-m,N), rfft axis [0,m)
@@ -255,9 +255,9 @@ class DistributedFNO(nn.Module):
     """Lift (time axis ``T_in->T_out``, channels ``C_in->width``), ``num_blocks`` Fourier
     layers, projection ``width->128->1``.  ``in_shape`` is the **global**
     ``[B, C_in, *spatial, T_in]``; the forward takes/returns this rank's ``P_x`` shard
-    (``/root/reference/dfno/dfno.py:293-353``).
+    (reference ``dfno/dfno.py:293-353``).
 
-    ``backend="auto"`` hands construction to the fused sm_100a engine when the device,
+    ``backend="auto"`` hands construction to the fused sm_90a engine when the device,
     dtype and partition are ones it covers (see :func:`dfno_b200.models.fused.supports`);
     ``backend="torch"`` forces this portable implementation.
     """
@@ -359,7 +359,7 @@ def infer_global_shape(P: Partition, local_shape: Sequence[int]) -> List[int]:
 
 class DistributedFNONd(nn.Module):
     """Keyword-style, lazily-shaped front end kept for scripts written against the older
-    API (``/root/reference/tests/gradient_test_dfno.py:11-26``): no ``in_shape`` -- it is
+    API (reference ``tests/gradient_test_dfno.py:11-26``): no ``in_shape`` -- it is
     inferred from the first input shard.  ``decomposition_order`` and ``P_y`` are accepted
     and ignored (the pencil plan is derived from ``P_x``)."""
 

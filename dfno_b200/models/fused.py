@@ -1,13 +1,13 @@
-"""Fused sm_100a engine for the model-parallel FNO (``backend="fused"``).
+"""Fused sm_90a engine for the model-parallel FNO (``backend="fused"``).
 
 Same function as :class:`dfno_b200.models.fno.DistributedFNO` (spec: SURVEY.md §3.1), but
-organised around B200 hardware instead of around ``torch.fft`` + MPI:
+organised around H100 hardware instead of around ``torch.fft`` + MPI:
 
 * **Layout.**  Activations live as ``h[b*C + c, x, y_local, t, z]`` in bf16 with ``z``
   contiguous.  The public tensors keep the reference layout ``[B, C, X, Y, Z, T]``; the lift
   and the projection head are the only places the layouts meet, so no transpose pass exists.
 * **Transforms are GEMMs.**  Each truncated (inverse) DFT stage is ``lines x K`` times a tiny
-  resident operator on tcgen05 (``csrc/dft_gemm_sm100.cu``), written by its epilogue directly
+  resident operator on wgmma (``csrc/dft_gemm_sm90.cu``), written by its epilogue directly
   in the layout -- and onto the GPU -- the next stage wants.  Complex data is interleaved
   (re, im) so a complex DFT is one real GEMM (``ops/operators.py``).
 * **Pencil transposes are fused.**  With the field split along ``y`` over ``P`` GPUs, stage m
@@ -24,7 +24,7 @@ organised around B200 hardware instead of around ``torch.fft`` + MPI:
 * **Backward is the same chain.**  The adjoint of every stage has the shape of its mirror
   stage, so the backward runs the identical kernel sequence with transposed operators.
 
-Reference call stack being replaced: ``/root/reference/dfno/dfno.py:241-291`` (block),
+Reference call stack being replaced: ``dfno/dfno.py:241-291`` of the reference package (block),
 ``:330-353`` (model).
 """
 from __future__ import annotations
@@ -45,9 +45,10 @@ from ..parallel.partition import Partition
 __all__ = ["FusedDistributedFNO", "FusedAdam", "supports", "wants", "EnginePlan", "fold_onto_pencil"]
 
 SUPPORTED_WIDTHS = (4, 8, 12, 16, 20, 24, 32)
-MAX_N = 256                  # n_pad limit of dft_gemm (TMEM accumulator columns per stage)
-HBM_BUDGET = 170 * 2 ** 30   # of a B200's 180 GB: leave room for the CUDA context, NCCL and the allocator
+MAX_N = 256                  # n_pad limit of dft_gemm (accumulator columns of one 64-row warpgroup tile)
+HBM_BUDGET = 72 * 2 ** 30    # of an H100's 80 GB: leave room for the CUDA context, NCCL and the allocator
 HEAD_HIDDEN = 128
+H100_COPY_GBS = 3027.0       # device-to-device copy bandwidth (GB/s, read + write) measured on an H100 80GB HBM3 at 700 W
 
 
 # =====================================================================================
@@ -101,7 +102,7 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
     split (e.g. BASELINE config 3's ``(1,1,2,2,2,1)`` or config 4's 8-way time partition) is served
     by re-sharding the (small) network input onto that pencil once, running the engine there and
     re-sharding the single-channel output back -- instead of the reference's two full-resolution
-    re-shards R1/R4 per Fourier layer (``/root/reference/dfno/dfno.py:247,288``).  5-D (2-D + time)
+    re-shards R1/R4 per Fourier layer (``dfno/dfno.py:247,288`` of the reference).  5-D (2-D + time)
     problems run as 6-D ones with a singleton x axis (:func:`_as_6d`)."""
     six = _as_6d(P_x.shape, in_shape, modes)
     if six is None:
@@ -122,7 +123,7 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
     if Cin > 4 or Tin > 64:
         return False, "lift kernel covers Cin <= 4 and Tin <= 64"
     # T % 4 != 0 (e.g. the reference's two-phase run and in-module demo, T = 30) uses a padded t pitch in Z1
-    # (EnginePlan.Tp); validated on a B200 in round 2 (tests/test_fused_gpu.py)
+    # (EnginePlan.Tp); covered by tests/test_fused_gpu.py
     if Z % 8 or T % 2 or Y % 4 or (X % 4 and X != 1) or (mx % 2 and X != 1) or my % 2 or mz % 2:
         return False, "extents must satisfy Z%8 = T%2 = X%4 = Y%4 = 0 and even modes (TMA pitch alignment)"
     if (X != 1 and 2 * mx > X) or 2 * my > Y or 2 * mz > Z or mt > T // 2 + 1:
@@ -344,7 +345,7 @@ class EnginePlan:
     def memory_bytes(self, train: bool = True, staged: Optional[bool] = None, legacy: bool = False) -> Dict[str, int]:
         """Per-rank device memory of the engine for this plan, by category (bytes).  Mirrors the
         allocations of :class:`FusedDistributedFNO` (``__init__``, ``_ensure_train_buffers``,
-        ``_ensure_eval_buffers``) and :class:`FusedAdam`; used to size shards for the 180 GB of a B200
+        ``_ensure_eval_buffers``) and :class:`FusedAdam`; used to size shards for the 80 GB of an H100
         before anything is allocated."""
         if self.num_blocks is None:
             raise RuntimeError("call finish(num_blocks) first")
@@ -373,16 +374,16 @@ class EnginePlan:
         out["total"] = sum(out.values())
         return out
 
-    def cost_model(self, hbm_gbs: float = 6491.8, nvlink_gbs: float = 770.0,
+    def cost_model(self, hbm_gbs: float = H100_COPY_GBS, nvlink_gbs: Optional[float] = None,
                    staged: Optional[bool] = None, legacy: bool = False, front: bool = False) -> Dict[str, object]:
         """Bytes every kernel of one training step must move (per rank) and the resulting floors.
         ``front``: G1a + G1b run as the single ``spectral_in`` kernel (Z1 stays on the SM).
 
         Pure bookkeeping of the dataflow in :class:`FusedDistributedFNO` -- each stage reads its input
         buffer and writes its output buffer once; nothing is assumed to stay in L2 (the working set of a
-        stage is far above 126 MB for the configurations this is meant for).  ``hbm_gbs`` / ``nvlink_gbs``
-        default to the measured copy bandwidth of ``MEASURED_PEAKS.json`` and the measured peer-copy
-        rate.  Returns ``{"stages": [(name, calls_per_step, hbm_bytes, nvlink_bytes)], "hbm_bytes",
+        stage is far above the 50 MB L2 for the configurations this is meant for).  ``hbm_gbs`` defaults to
+        the device-to-device copy bandwidth measured on an H100 (:data:`H100_COPY_GBS`); without
+        ``nvlink_gbs`` the NVLink time is not estimated (``nvlink_ms`` is None).  Returns ``{"stages": [(name, calls_per_step, hbm_bytes, nvlink_bytes)], "hbm_bytes",
         "nvlink_bytes", "hbm_floor_ms", "nvlink_ms"}``; the NVLink time is overlappable (the transfers are
         issued from GEMM epilogues), so the step floor is ``max`` of the two per chain, not their sum."""
         if self.num_blocks is None:
@@ -425,7 +426,7 @@ class EnginePlan:
         link = sum(c * l for _, c, _, l in st)
         return {"stages": st, "hbm_bytes": hbm, "nvlink_bytes": link,
                 "hbm_floor_ms": hbm / (hbm_gbs * 1e9) * 1e3,
-                "nvlink_ms": link / (nvlink_gbs * 1e9) * 1e3 if link else 0.0}
+                "nvlink_ms": (link / (nvlink_gbs * 1e9) * 1e3 if link else 0.0) if nvlink_gbs else None}
 
     def operators(self) -> Dict[str, torch.Tensor]:
         """Forward-chain operators (float64) and their adjoint-chain counterparts (``*_adj``)."""
@@ -521,7 +522,7 @@ class _FusedFn(torch.autograd.Function):
 
 
 class FusedDistributedFNO(nn.Module):
-    """Drop-in ``DistributedFNO`` on the fused sm_100a engine.  Same constructor; the forward
+    """Drop-in ``DistributedFNO`` on the fused sm_90a engine.  Same constructor; the forward
     takes this rank's ``[B, C_in, X, Y_local, Z, T_in]`` shard (fp32 or bf16, CUDA) and returns
     ``[B, 1, X, Y_local, Z, T_out]`` in fp32."""
 
@@ -597,9 +598,8 @@ class FusedDistributedFNO(nn.Module):
         self._saved: Dict[str, torch.Tensor] = {}
         self._train_bufs_ready = False
         self._generation = 0                     # number of saving forwards so far (see _FusedFn)
-        # staged peer layout (long NVLink runs + local permutation): measured win at 8 GPUs (exposed
-        # all-to-all 0.19 -> 0.08 ms per chain), measured loss at 2 (the permutation costs more than the
-        # 40-/256-byte runs did); "auto" = on from 8 ranks.
+        # staged peer layout (long NVLink runs + a local permutation): it pays when the direct runs get short,
+        # i.e. with many ranks, and costs a permutation pass with few; "auto" = on from 8 ranks.
         _st = os.environ.get("DFNO_STAGED_SCATTER", "auto").lower()
         mode = (self.world >= 8) if _st == "auto" else (_st if _st in ("r2", "r3") else _st != "0")
         self.staged_scatter = mode if self.world > 1 else False      # False / True / "r2" / "r3"
@@ -613,11 +613,11 @@ class FusedDistributedFNO(nn.Module):
             self.ws["T1"] = torch.zeros(pl.n_T1, **bf)
         self.use_tc_bypass = (pl.S % 128 == 0 and pl.C <= 32 and os.environ.get("DFNO_TC_BYPASS", "1") != "0")
         # round-2 dataflow: the last GEMM of every chain also applies the bypass conv (+ GELU), and the head reads
-        # the channel-major activation directly (csrc/spectral_out_sm100.cu, dpre_dw_sm100.cu, head_sm100.cu).
+        # the channel-major activation directly (csrc/spectral_out_sm90.cu, dpre_dw_sm90.cu, head_sm90.cu).
         # DFNO_POINTWISE=legacy keeps round 1's separate bypass / channels-last head kernels for A/B runs.
         self.fused_pw = os.environ.get("DFNO_POINTWISE", "fused").lower() != "legacy" and 2 * pl.KZ <= 128
         # the first two GEMMs of every chain (z-DFT, t-DFT) + the transpose R2 as ONE kernel that keeps Z1 on the SM
-        # (csrc/spectral_in_sm100.cu); DFNO_FRONT=legacy keeps the two dft_gemm launches for A/B runs.
+        # (csrc/spectral_in_sm90.cu); DFNO_FRONT=legacy keeps the two dft_gemm launches for A/B runs.
         self.front = None
         if os.environ.get("DFNO_FRONT", "fused").lower() != "legacy":
             self.front = self._front_plan()
@@ -661,7 +661,7 @@ class FusedDistributedFNO(nn.Module):
         return base[off:off + int(np.prod(shape))].view(shape)
 
     def _init_parameters(self, seed: Optional[int] = None) -> None:
-        """Reference initialisation (``/root/reference/dfno/dfno.py:35-36,114-117,160``): Kaiming-uniform pointwise
+        """Reference initialisation (reference ``dfno/dfno.py:35-36,114-117,160``): Kaiming-uniform pointwise
         weights, zero biases, ``U[0,1)/C^2`` spectral weights.  With ``seed`` the draw is *partition independent*:
         pointwise weights come from one generator seeded identically on every rank and every retained ``kz`` slab
         of every block from its own generator seeded by its GLOBAL index, so 1, 2, 4 and 8 ranks build the same
@@ -820,7 +820,7 @@ class FusedDistributedFNO(nn.Module):
         return w3a, w3t
 
     def _wpad(self, W: torch.Tensor) -> torch.Tensor:
-        """[C, C] fp32 -> zero-padded bf16 [32, 64] tcgen05 operand (rows = output index)."""
+        """[C, C] fp32 -> zero-padded bf16 [32, 64] wgmma operand (rows = output index)."""
         out = torch.zeros(32, 64, device=self.device, dtype=torch.bfloat16)
         out[:W.shape[0], :W.shape[1]] = W.to(torch.bfloat16)
         return out
@@ -838,7 +838,7 @@ class FusedDistributedFNO(nn.Module):
         return [pl.Z, pl.T, pl.B * pl.X * pl.Yl], [pl.T, 1, pl.Z * pl.T]
 
     def _head_forward(self, hcl: torch.Tensor) -> torch.Tensor:
-        """linear3 -> gelu -> linear4 in the epilogue of one tcgen05 GEMM (EPI_HEAD)."""
+        """linear3 -> gelu -> linear4 in the epilogue of one wgmma GEMM (EPI_HEAD)."""
         pl = self.plan
         w3, _ = self._head_operators()
         out = torch.empty(pl.B, 1, pl.X, pl.Yl, pl.Z, pl.T, device=self.device, dtype=torch.float32)
@@ -958,7 +958,7 @@ class FusedDistributedFNO(nn.Module):
                 Wb = self._seg(f"blocks.{k}.linear.W")
                 gW = self._seg(f"blocks.{k}.linear.W", self.grad_flat)
                 if self.use_tc_bypass:
-                    # one tcgen05 kernel: dpre (over pre), dhb = W^T dpre, dW accumulated in TMEM
+                    # one wgmma kernel: dpre (over pre), dhb = W^T dpre, dW accumulated in registers
                     C_.bypass_bwd_tc(None if last else g, gcl if last else None, pl.CP, pres[k], hs[k],
                                      self._wpad(Wb.t()), dhb, gW, pl.B, pl.C, pl.S)
                 else:

@@ -4,7 +4,7 @@
 axis of an N-D field shard.  The parameters live **only on rank 0 of ``P_x``**; other ranks
 hold zero-volume parameters (so optimizers and checkpoints see the same key set
 everywhere).  Forward broadcasts ``W``/``b``; the autograd adjoint sum-reduces their
-gradients back onto the root.  Spec: ``/root/reference/dfno/dfno.py:17-65``.
+gradients back onto the root.  Spec: reference ``dfno/dfno.py:17-65``.
 
 Differences by design: the bias parameter is only materialised when ``bias=True`` is
 requested *or* ``ref_state_dict=True`` (checkpoint parity with the reference, which always
@@ -53,7 +53,7 @@ class BroadcastedLinear(nn.Module):
         self.W_bcast.link.meta = ((self.out_features, self.in_features), dtype)
         self.b_bcast.link.meta = (tuple(self.b_shape), dtype)
         # the contraction in einsum notation ("oi,ab..i..->ab..o.."), kept as an attribute for API
-        # parity (/root/reference/dfno/dfno.py:44-49); the forward uses movedim + matmul instead
+        # parity (reference dfno/dfno.py:44-49); the forward uses movedim + matmul instead
         letters = "abcdefghjklmnpqrstuvwxyz"[:P_x.dim]
         lhs = letters[:self.dim] + "i" + letters[self.dim + 1:]
         self.eqn = f"oi,{lhs}->{lhs.replace('i', 'o')}"
@@ -80,5 +80,5 @@ class BroadcastedLinear(nn.Module):
         return y
 
 
-#: stale name imported by ``/root/reference/tests/gradient_test_distdl.py:7``
+#: stale name imported by reference ``tests/gradient_test_distdl.py:7``
 BroadcastedAffineOperator = BroadcastedLinear

@@ -5,7 +5,7 @@ Broadcast), so the scalar is *valid on the root rank* and a differentiable ``0``
 -- every rank can call ``loss.backward()``.
 
 * ``DistributedRelativeLpLoss``: batch mean of ``||y^-y||_p / ||y||_p`` with the norms taken
-  over the whole (global) sample -- ``/root/reference/dfno/loss.py:8-35``.
+  over the whole (global) sample -- reference ``dfno/loss.py:8-35``.
 * ``DistributedMSELoss``: global mean squared error (DistDL module the reference's
   scripts use: ``experiment_navier_stokes.py:118``, ``dfno.py:374``; SURVEY.md §2.2 E6).
 """
@@ -35,7 +35,7 @@ class _EngineReducedLoss(torch.autograd.Function):
     all-reduce of the 2B partial sums, CUDA-graph capturable, value valid on *every* rank) or ``None`` for a
     partition of one rank.  On fp32 CUDA fields the forward is one pass over ``y_hat`` and ``y`` and the backward
     one pass writing the gradient (``csrc/loss.cu``) -- the autograd graph of the reference formulation
-    (``/root/reference/dfno/loss.py:8-35``) launches eight elementwise / reduction kernels and keeps the
+    (reference ``dfno/loss.py:8-35``) launches eight elementwise / reduction kernels and keeps the
     difference field alive between them."""
 
     @staticmethod

@@ -1,7 +1,7 @@
 """Batch normalisation over a domain-decomposed field.
 
 The reference constructs two ``DistributedBatchNorm(P_x, width)`` modules and leaves them
-out of the forward (``/root/reference/dfno/dfno.py:325-326,340,346``); they matter only for
+out of the forward (reference ``dfno/dfno.py:325-326,340,346``); they matter only for
 ``state_dict()`` parity.  This is a complete implementation nonetheless (per-channel
 statistics all-reduced over ``P_x`` so every shard normalises with the global mean and
 variance), usable by models that want it.

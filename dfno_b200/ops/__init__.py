@@ -1,1 +1,1 @@
-"""Python wrappers (autograd, planning) around the sm_100a kernels in ``dfno_b200/csrc``."""
+"""Python wrappers (autograd, planning) around the sm_90a kernels in ``dfno_b200/csrc``."""

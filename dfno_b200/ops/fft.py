@@ -7,7 +7,7 @@ un-truncated transforms, power-of-two axes up to 4096 samples -- and what the po
 built with ``fft_impl="native"`` (no cuFFT on that path).  Complex data is interleaved ``[..., n, 2]``
 (``torch.view_as_real`` layout); fp32 or bf16 storage, fp32 arithmetic.  CPU tensors, other dtypes and
 non-power-of-two lengths fall back to ``torch.fft`` with identical semantics
-(reference ops: ``/root/reference/dfno/dfno.py:252-258,273-285``)."""
+(reference ops: reference ``dfno/dfno.py:252-258,273-285``)."""
 from __future__ import annotations
 
 import torch

@@ -1,4 +1,4 @@
-"""Python front end of the resident-operator tcgen05 GEMM (``csrc/dft_gemm_sm100.cu``)."""
+"""Python front end of the resident-operator wgmma GEMM (``csrc/dft_gemm_sm90.cu``)."""
 from __future__ import annotations
 
 from typing import List, Optional, Sequence, Tuple

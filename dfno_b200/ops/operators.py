@@ -4,7 +4,7 @@ Every stage of the distributed spectral convolution is ``out = A @ Op^T`` with `
 field viewed as ``[lines, K]`` and ``Op`` one of the matrices below (built in float64,
 rounded to bf16 for the tensor cores).  Conventions are ``torch.fft``'s: forward unscaled,
 inverse scaled by ``1/N``; the retained modes of a two-sided axis are ``[0, m) u [N-m, N)``
-in that order, of the one-sided (rfft) axis ``[0, m)`` (``/root/reference/dfno/dfno.py:104-111``).
+in that order, of the one-sided (rfft) axis ``[0, m)`` (reference ``dfno/dfno.py:104-111``).
 
 Because complex numbers are stored as adjacent (re, im) pairs, a complex DFT is ONE real
 GEMM against ``[[c, s], [-s, c]]`` blocks -- no 3M trick, no de-interleave pass.  The

@@ -3,7 +3,7 @@
 This is the arithmetic every other layer (Repartition plans, spectral-weight shards,
 checkpoint layout, the per-rank dataset slabs) is built on.  The rule is the one the
 reference inherits from DistDL (contract described in SURVEY.md §2.2 E9 and used at
-``/root/reference/dfno/utils.py:58-70`` and ``training/two_phase/sleipner_dataset.py:51-52``):
+reference ``dfno/utils.py:58-70`` and ``training/two_phase/sleipner_dataset.py:51-52``):
 a length ``n`` axis split over ``p`` workers gives the first ``n mod p`` workers
 ``ceil(n/p)`` entries and the rest ``floor(n/p)``.
 

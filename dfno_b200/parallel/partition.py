@@ -4,7 +4,7 @@ A :class:`Partition` is an ordered set of world ranks arranged on an N-D worker 
 (row-major).  It is the object every distributed layer takes as ``P_x`` and the public
 workflow starts from :func:`create_standard_partitions`.  It plays the role DistDL's MPI
 ``Partition`` plays for the reference (contract: SURVEY.md §2.2 E1; call sites
-``/root/reference/dfno/utils.py:72-83``, ``/root/reference/dfno/dfno.py:83-97``) but is
+reference ``dfno/utils.py:72-83``, reference ``dfno/dfno.py:83-97``) but is
 built for one-process-per-GPU on a single NVSwitch box:
 
 * rendezvous/control plane is ``torch.distributed`` (NCCL on GPU, gloo on CPU);
@@ -59,7 +59,7 @@ def reset_group_cache() -> None:
 
 class _CommShim:
     """Minimal stand-in for the raw communicator scripts reach through ``P._comm``
-    (``Barrier`` at ``/root/reference/dfno/dfno.py:384``; ``allreduce`` MIN/MAX at
+    (``Barrier`` at reference ``dfno/dfno.py:384``; ``allreduce`` MIN/MAX at
     ``training/two_phase/sleipner_dataset.py:93,96``)."""
 
     def __init__(self, part: "Partition"):
@@ -206,7 +206,7 @@ def _default_device() -> torch.device:
 
 
 def create_root_partition(P: Partition) -> Partition:
-    """Rank 0 of ``P`` as a ``[1]*dim`` grid (``/root/reference/dfno/utils.py:72-75``)."""
+    """Rank 0 of ``P`` as a ``[1]*dim`` grid (reference ``dfno/utils.py:72-75``)."""
     return P.create_partition_inclusive([0]).create_cartesian_topology_partition([1] * P.dim)
 
 
@@ -214,7 +214,7 @@ def create_standard_partitions(shape: Sequence[int]):
     """``(P_world, P_x, P_root)`` for a worker grid ``shape``.
 
     ``P_x`` spans the first ``prod(shape)`` world ranks (row-major on the grid) and
-    ``P_root`` is its rank 0 (``/root/reference/dfno/utils.py:77-83``).  If
+    ``P_root`` is its rank 0 (reference ``dfno/utils.py:77-83``).  If
     ``torch.distributed`` has not been initialised but the launcher environment
     (``RANK``/``WORLD_SIZE``) is present, the process group is created here: NCCL when CUDA
     is available, gloo otherwise.

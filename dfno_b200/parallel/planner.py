@@ -8,7 +8,7 @@ transform is done in two local stages separated by global re-shards:
     P_y --R3--> P_m --R4--> P_x on the way back.
 
 ``plan="reference"`` reproduces the worker-grid arithmetic of
-``/root/reference/dfno/dfno.py:82-97`` exactly (needed for checkpoint-layout parity; note
+reference ``dfno/dfno.py:82-97`` exactly (needed for checkpoint-layout parity; note
 its quirk for an odd number of transformed axes, SURVEY.md §5.7 item 5: ranks are left
 idle in stage y).  ``plan="balanced"`` is this framework's own choice for stage y: all
 workers are spread over the *retained-mode* extents of the stage-m axes so that no rank
@@ -115,7 +115,7 @@ def corner_boxes(spec_shape: Sequence[int], modes: Sequence[int], start: Sequenc
     transformed axis is the least significant digit; 0 = low modes ``[0,m)``, 1 = high modes ``[size-m,size)``), the
     non-empty intersections as per-axis ``(a, b)`` *local* bounds for axes ``2..``.  This
     is the enumeration that fixes the ``weights.{j}`` checkpoint keys
-    (``/root/reference/dfno/dfno.py:137-161``).
+    (reference ``dfno/dfno.py:137-161``).
     """
     nd = len(spec_shape)
     n = nd - 2

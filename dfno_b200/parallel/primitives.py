@@ -3,9 +3,9 @@
 ``Broadcast`` / ``SumReduce`` are an adjoint pair, ``Repartition`` is its own adjoint
 family (adjoint of ``P_a -> P_b`` is ``P_b -> P_a``).  These are the torch.distributed
 (gloo / NCCL) implementations: they are the CPU path, the functional fallback for any
-partition the fused sm_100a engine does not cover, and -- run over NCCL -- the measured
+partition the fused sm_90a engine does not cover, and -- run over NCCL -- the measured
 baseline.  Contracts follow SURVEY.md §2.2 (E2, E3, E4, E7, E8); reference call sites are
-``/root/reference/dfno/dfno.py:41-42,57-58,99-102`` and ``/root/reference/dfno/loss.py:17-35``.
+reference ``dfno/dfno.py:41-42,57-58,99-102`` and reference ``dfno/loss.py:17-35``.
 
 Conventions
 -----------
@@ -220,7 +220,7 @@ class AllSumReduce(nn.Module):
 class ZeroVolumeCorrectorFunction(torch.autograd.Function):
     """Turn a zero-volume result into a scalar 0 so every rank
     can call ``.backward()``; the backward hands the original empty shape back.
-    (contract: SURVEY.md §2.2 E7, used at ``/root/reference/dfno/loss.py:35``)."""
+    (contract: SURVEY.md §2.2 E7, used at reference ``dfno/loss.py:35``)."""
 
     @staticmethod
     def forward(ctx, x):

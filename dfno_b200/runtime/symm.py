@@ -4,7 +4,7 @@
 the ``torch.distributed`` control plane and maps every peer's allocation, yielding
 ``ptrs[r]`` = a device pointer *valid on this GPU* to rank ``r``'s buffer.  Kernels store to /
 load from those pointers directly (NVSwitch routes the traffic); see ``csrc/symm_mem.cpp``,
-``csrc/p2p.cu`` and the peer-scatter epilogue of ``csrc/dft_gemm_sm100.cu``.
+``csrc/p2p.cu`` and the peer-scatter epilogue of ``csrc/dft_gemm_sm90.cu``.
 """
 from __future__ import annotations
 

@@ -1,7 +1,7 @@
 """Training-step driver: host batch -> device (pinned, asynchronous, double buffered) ->
 forward -> distributed loss -> backward -> optimizer, loss read back to the host.
 
-This is the loop of ``/root/reference/training/two_phase/train_two_phase.py:99-121`` as a
+This is the loop of reference ``training/two_phase/train_two_phase.py:99-121`` as a
 reusable object.  The H2D copies of step ``i+1`` run on a side stream while step ``i``
 computes; the loss value is read back from a pinned scalar.
 """
@@ -187,7 +187,7 @@ class Trainer:
 class InferenceSession:
     """Forward-only serving loop: pinned host shard in -> (CUDA-graph replayed) forward -> pinned host
     shard out.  The counterpart of :class:`Trainer` for deployment; the reference only has the one-shot
-    script ``/root/reference/training/two_phase/test_two_phase.py``.
+    script reference ``training/two_phase/test_two_phase.py``.
 
     ``run`` is synchronous (returns when the output is on the host); ``submit`` / ``result`` split it so
     that the upload of request ``i+1`` overlaps the forward of request ``i``.  With ``cuda_graph`` the

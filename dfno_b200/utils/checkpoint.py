@@ -6,7 +6,7 @@ Two formats:
   ``model_{rank:04d}.pt`` holding ``state_dict()`` of that rank -- root-owned pointwise
   weights are real tensors on rank 0 and zero-volume elsewhere, spectral weights are one
   tensor per non-empty corner of the rank's ``P_y`` slab
-  (``/root/reference/training/two_phase/train_two_phase.py:163-169``).  Only loadable on the
+  (reference ``training/two_phase/train_two_phase.py:163-169``).  Only loadable on the
   same partition.  This module additionally writes optimizer state, RNG state and
   epoch/step counters next to it so training can *resume* (the reference cannot).
 * **global / canonical** (new): one partition-independent dict -- full pointwise weights and,

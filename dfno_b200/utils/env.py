@@ -1,7 +1,7 @@
 """Process/bootstrap helpers: process-group creation from the launcher environment,
 device selection (``get_env``), seeding.
 
-Reference: ``/root/reference/dfno/utils.py:42-55`` selects CPU / host-staged GPU /
+Reference: reference ``dfno/utils.py:42-55`` selects CPU / host-staged GPU /
 CUDA-aware MPI from ``USE_CUDA`` / ``CUDA_AWARE``.  Here there is one data path per device
 type -- gloo for CPU tensors, NCCL + NVLink peer memory for CUDA tensors -- so the two
 variables only decide *whether* the GPU is used.

@@ -3,7 +3,7 @@
 For every parameter ``p`` with a random direction ``dp`` the zeroth-order remainder
 ``|J(p+h dp) - J(p)|`` must decay like ``h`` and the first-order remainder
 ``|J(p+h dp) - J(p) - h <grad J, dp>|`` like ``h^2``; slopes are fitted in log-log space.
-Same idea as ``/root/reference/tests/gradient_test.py:40-132``, with the distributed
+Same idea as reference ``tests/gradient_test.py:40-132``, with the distributed
 details done properly:
 
 * the objective is the **global** ``1/2 ||f(x) - y0||^2`` (local terms all-reduced), not a

@@ -1,7 +1,7 @@
 """Rank-aware console output and a JSON-lines metrics sink.
 
 The reference only ``print``s: a ``print0`` helper in its benchmark (root rank only,
-``/root/reference/benchmarks/bench.py:26-29``), per-batch losses and wall times in the trainers
+reference ``benchmarks/bench.py:26-29``), per-batch losses and wall times in the trainers
 (``train_two_phase.py:121,150``).  Here the same information goes through one small layer so that
 every line is tagged with its rank and every number also lands in a machine-readable file."""
 from __future__ import annotations

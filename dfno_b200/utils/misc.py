@@ -1,4 +1,4 @@
-"""Small utilities of the public namespace (``/root/reference/dfno/utils.py``)."""
+"""Small utilities of the public namespace (reference ``dfno/utils.py``)."""
 from __future__ import annotations
 
 import subprocess
@@ -78,7 +78,7 @@ def get_gpu_memory():
 
 def profile_gpu_memory(outfile, dt: float = 1.0, max_samples: int = None):
     """Poll :func:`get_gpu_memory` every ``dt`` seconds into a CSV (meant for a daemon
-    process, ``/root/reference/benchmarks/bench.py:57-62``)."""
+    process, reference ``benchmarks/bench.py:57-62``)."""
     t0 = time.time()
     n = 0
     with open(outfile, "w") as f:

@@ -1,7 +1,7 @@
 """Timing helpers.
 
 ``CommTimer`` reproduces the reference's per-module ``dt_comm`` accounting
-(``/root/reference/dfno/dfno.py:54-60,242-289``) but can be told to synchronise the device so
+(reference ``dfno/dfno.py:54-60,242-289``) but can be told to synchronise the device so
 the number means something on an asynchronous GPU stream.  ``cuda_time_ms`` is the
 benchmark-grade device timer (CUDA events, explicit synchronisation on both sides).
 """

@@ -5,7 +5,7 @@ from setuptools import find_packages, setup
 setup(
     name="dfno_b200",
     version="0.1.0",
-    description="Blackwell-native model-parallel Fourier Neural Operators (dfno-compatible API)",
+    description="Hopper-native model-parallel Fourier Neural Operators (dfno-compatible API)",
     packages=find_packages(include=["dfno_b200*", "dfno"]),
     package_data={"dfno_b200": ["csrc/*"]},
     python_requires=">=3.10",

@@ -1,4 +1,4 @@
-"""tcgen05 resident-operator GEMM vs a plain fp32 PyTorch reference (B200 only)."""
+"""wgmma resident-operator GEMM vs a plain fp32 PyTorch reference (H100 only)."""
 import numpy as np
 import pytest
 import torch

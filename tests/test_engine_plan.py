@@ -221,7 +221,7 @@ def test_memory_plan_sizes_shards_for_a_b200():
     ok, why = supports(_Grid(1, 1, 1, 1, 1, 1), [8, 1, 128, 128, 128, 1], 20, 20, (12, 12, 12, 10))
     assert not ok and ("GiB" in why or "2^31" in why)
     assert supports(_Grid(1, 1, 1, 8, 1, 1), [8, 1, 128, 128, 128, 1], 20, 20, (12, 12, 12, 10))[0]
-    assert HBM_BUDGET < 180 * 2 ** 30
+    assert HBM_BUDGET < 80 * 2 ** 30                                    # an H100 holds 80 GB
 
 
 def test_column_parts_address_the_same_elements():
@@ -257,10 +257,9 @@ def test_column_parts_address_the_same_elements():
 
 
 def test_cost_model_reproduces_measured_dram_traffic():
-    """The per-kernel byte counts of the traffic model against the DRAM bytes ncu measured on a B200 for the
-    headline configuration (RESULTS.md, profiles/r1_ncu_*.json, launch list v3 for the round-1 dataflow;
-    profiles/r2_launch_list_fused_1gpu.csv for the fused pointwise dataflow) -- within 8 % (the small stages see
-    some L2 hits; 12 % for spectral_out, whose U input is partly still in the 126 MB L2)."""
+    """The per-kernel byte counts of the traffic model against the DRAM bytes Nsight Compute recorded for the
+    headline configuration on a B200 (126 MB L2), not re-recorded on an H100: the bytes a kernel must move belong
+    to the dataflow; the tolerance (8 %, 12 % for spectral_out) covers that device's L2 hits."""
     pl = EnginePlan(1, 1, 1, 20, 20, 128, 128, 128, (12, 12, 12, 10), world=1, rank=0)
     pl.finish(4)
     cm = pl.cost_model(legacy=True)
@@ -269,17 +268,17 @@ def test_cost_model_reproduces_measured_dram_traffic():
                    "spectral_mix fwd": 0.46, "spectral_mix bwd": 0.87, "adam": 12.3, "head fwd": 2.2, "head bwd": 4.2}
     for k, v in measured_gb.items():
         assert abs(got[k] - v) / v < 0.08, (k, got[k], v)
-    assert 20.0 < cm["hbm_floor_ms"] < 27.0 and cm["nvlink_bytes"] == 0
+    assert 130e9 < cm["hbm_bytes"] < 175e9 and cm["nvlink_bytes"] == 0
     cm = pl.cost_model()                                   # round-2 dataflow: fused pointwise kernels
     got = {n: b / 1e9 for n, _, b, _ in cm["stages"]}
     measured_gb = {"G1a": 2.274, "G1b": 0.910, "G2": 0.354, "iG1b": 0.952, "spectral_out fwd": 5.624, "dpre_dw": 6.852,
                    "head fwd": 1.835, "head bwd": 3.483 + 0.168, "adam": 12.33, "lift fwd": 1.622, "lift bwd": 1.686}
     for k, v in measured_gb.items():
         assert abs(got[k] - v) / v < (0.12 if k == "spectral_out fwd" else 0.08), (k, got[k], v)
-    assert 15.0 < cm["hbm_floor_ms"] < 21.0 and cm["nvlink_bytes"] == 0
+    assert 97.4e9 < cm["hbm_bytes"] < 136e9 and cm["nvlink_bytes"] == 0
     cf = pl.cost_model(front=True)                         # + spectral_in: Z1 (0.63 GB written and re-read) is gone
     assert abs((cm["hbm_bytes"] - cf["hbm_bytes"]) - 8 * 2 * pl.n_Z1 * 2) < 1e6
-    assert cf["hbm_floor_ms"] < cm["hbm_floor_ms"] - 1.4
+    assert cf["hbm_bytes"] < cm["hbm_bytes"] - 9.1e9
     p8 = EnginePlan(1, 1, 1, 20, 20, 128, 128, 128, (12, 12, 12, 10), world=8, rank=0)
     p8.finish(4)
     assert p8.cost_model(front=True)["nvlink_bytes"] == p8.cost_model()["nvlink_bytes"]
@@ -289,7 +288,7 @@ def test_cost_model_reproduces_measured_dram_traffic():
 
 
 def test_fused_front_stage_plan_and_eligibility():
-    """Host-side tile planner of csrc/spectral_in_sm100.cu (no GPU needed): the configurations the engine relies
+    """Host-side tile planner of csrc/spectral_in_sm90.cu (no GPU needed): the configurations the engine relies
     on are accepted with the expected tile shape, and the documented limits are refused with a reason (the engine
     then keeps the two separate GEMMs)."""
     from dfno_b200.ops import build
@@ -302,10 +301,11 @@ def test_fused_front_stage_plan_and_eligibility():
         why = C_.spectral_in_check(*a)
         return why, (C_.spectral_in_config(*a) if not why else None)
 
-    # headline, one rank: S1[bc, kz, kt, x, y, ri]; 4 positions per tile, 32-position store chunks, 4 groups
+    # headline, one rank: S1[bc, kz, kt, x, y, ri]; 4 positions per tile, 32-position store chunks, 2 consumer
+    # warpgroups
     Y = 128
     why, c = cfg(1, 0, [Y * 2, 128 * Y * 2, 10 * 128 * Y * 2, 24 * 10 * 128 * Y * 2], 20, 128, 128, 20, 128, 24, 10)
-    assert why == "" and c[:3] == [4, 32, 4] and c[3] >= 4
+    assert why == "" and c[:3] == [4, 32, 2] and c[3] >= 4
     # headline, rank 5 of 8, staged layout S1s[bc, kz', kt, r_src, x, y_loc, ri]: 16 local y -> 16-position chunks
     P, Yl, X = 8, 16, 128
     dstr = [Yl * 2, P * X * Yl * 2, 10 * P * X * Yl * 2, 3 * 10 * P * X * Yl * 2]
@@ -327,7 +327,7 @@ def test_fused_front_stage_plan_and_eligibility():
 
 
 def _emulate_spectral_in(h, o1, o2, dst, dst_off, dstr, BC, X, Yl, T, Z, KZ, mt, P, Rp, Yc):
-    """Float64 replay of csrc/spectral_in_sm100.cu with the kernel's own index arithmetic: tiles of Rp positions,
+    """Float64 replay of csrc/spectral_in_sm90.cu with the kernel's own index arithmetic: tiles of Rp positions,
     D1 -> A2 transposition, D2 -> staging[kz][kt][y], one clipped box store per destination rank and chunk."""
     kzl, tpc, ncy = KZ // P, Yc // Rp, (Yl + Yc - 1) // Yc
     lines = h.reshape(BC * X, Yl * T, Z)

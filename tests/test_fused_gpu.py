@@ -1,4 +1,4 @@
-"""Fused sm_100a engine vs the portable fp32 backend on one B200."""
+"""Fused sm_90a engine vs the portable fp32 backend on one H100."""
 import pytest
 import torch
 

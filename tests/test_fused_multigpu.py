@@ -1,4 +1,4 @@
-"""Fused engine over ALL visible B200s (2, 4 or 8 ranks): NVLink peer-scatter epilogues (R2 / R3) in every
+"""Fused engine over ALL visible H100s (2, 4 or 8 ranks): NVLink peer-scatter epilogues (R2 / R3) in every
 layout (direct, staged, staged for one transpose only), device flag barrier, peer-memory gradient / loss
 all-reduce, general partitions folded onto the pencil (BASELINE configs 3 and 4 in miniature) and the 2-D + time
 plan -- each against the fp32 portable backend evaluated on the whole field.

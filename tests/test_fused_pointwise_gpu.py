@@ -1,5 +1,5 @@
 """Round-2 fused pointwise kernels (packed-fp16 GELU, spectral_out, dpre_dw, channel-major projection head)
-against plain PyTorch fp32 references of the same ops (B200 only)."""
+against plain PyTorch fp32 references of the same ops (H100 only)."""
 import math
 
 import pytest

@@ -1,4 +1,4 @@
-"""Peer-memory data plane on several B200s: push all-to-all-v vs NCCL, Repartition over it
+"""Peer-memory data plane on several H100s: push all-to-all-v vs NCCL, Repartition over it
 (values + adjoint), flag barrier and small all-reduce."""
 import numpy as np
 import pytest

@@ -1,75 +1,72 @@
-"""The UNMODIFIED reference package (``baseline/_ref/dfno``, installed with ``pip --no-deps`` from
-``/root/reference``) against this framework, from the same weights.
+"""This framework against the UNMODIFIED reference package (slimgroup/dfno), from the same weights.
 
-The reference cannot import on its own here (DistDL / mpi4py are not installable offline); it runs on
-the import-surface layer in ``baseline/compat`` that forwards DistDL's primitives to
-``dfno_b200.parallel``.  Everything else on the reference side -- model code, einsums, restrict /
-zeropad / ``torch.fft`` calls, per-forward weight broadcasts, the loss -- is the reference's own.
-Checked: identical state-dict keys and per-rank shard shapes, outputs, loss and gradients on 1 and
-4 ranks (``(1,1,2,2,1,1)``, the reference's in-module demo grid, ``/root/reference/dfno/dfno.py:359``)."""
+``tests/golden/reference_parity.npz`` holds what the reference computed for the cases below, recorded once by
+running its own code (on the DistDL / mpi4py stand-in in ``baseline/compat``) with every real or complex
+floating-point state-dict entry replaced by the seeded values of :func:`_seeded_state_dict`: per rank, the
+reference's state-dict shapes and distribution info, its output, loss (root rank) and parameter gradients.
+``oracle/gen_reference_parity.py`` (after ``oracle/install_reference.sh``) records it again.
+Checked: identical state-dict keys and per-rank shard shapes, outputs, loss and gradients on 1, 2 and 4 ranks
+(``(1,1,2,2,1,1)`` is the reference's in-module demo grid, ``dfno/dfno.py:359`` of the reference)."""
 import os
-import sys
 
+import numpy as np
 import pytest
 import torch
 
 from dfno_b200.utils.testing import run_distributed
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
-COMPAT = os.path.join(ROOT, "baseline", "compat")
-
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "dfno")),
-                                reason="reference package not installed under baseline/_ref")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_parity.npz")
 
 
-def _import_reference():
-    for p in (REF, COMPAT):
-        if p in sys.path:
-            sys.path.remove(p)
-    sys.path[:0] = [COMPAT, REF]
-    sys.modules.pop("dfno", None)
-    import dfno as ref
-    assert os.path.abspath(ref.__file__).startswith(REF), ref.__file__
-    return ref
+def _seeded_state_dict(sd, rank):
+    """Every real or complex floating-point entry of ``sd`` replaced by seeded normal values (scale 0.3, keys in
+    sorted order)."""
+    out = {}
+    for i, k in enumerate(sorted(sd)):
+        v = sd[k]
+        if v.is_floating_point() or v.is_complex():
+            g = torch.Generator().manual_seed(1000 * (rank + 1) + i)
+            v = 0.3 * torch.randn(v.shape, dtype=v.dtype, generator=g)
+        out[k] = v
+    return out
 
 
 def _parity(rank, ws, grid, in_shape, nt, width, modes, blocks):
     import warnings
     warnings.filterwarnings("ignore")
-    ref = _import_reference()
     import dfno_b200 as d
-    _, P_ref, _ = ref.create_standard_partitions(grid)
+    gold = np.load(GOLDEN)
+    pre = f"ws{ws}/r{rank}/"
     _, P_x, _ = d.create_standard_partitions(grid)
-    torch.manual_seed(10 + rank)
-    theirs = ref.DistributedFNO(P_ref, in_shape, nt, width, modes, num_blocks=blocks, dtype=torch.float64)
     ours = d.DistributedFNO(P_x, in_shape, nt, width, modes, num_blocks=blocks, dtype=torch.float64,
                             backend="torch", plan="reference")
-    sd = theirs.state_dict()
-    assert sorted(sd) == sorted(ours.state_dict()), "state-dict keys differ"
-    for k, v in ours.state_dict().items():
-        assert tuple(v.shape) == tuple(sd[k].shape), (k, tuple(v.shape), tuple(sd[k].shape))
-    ours.load_state_dict(sd)
+    sd = ours.state_dict()
+    ref_keys = sorted(k[len(pre + "sdshape/"):] for k in gold.files if k.startswith(pre + "sdshape/"))
+    assert sorted(sd) == ref_keys, "state-dict keys differ"
+    for k, v in sd.items():
+        want = tuple(int(s) for s in gold[pre + "sdshape/" + k])
+        assert tuple(v.shape) == want, (k, tuple(v.shape), want)
+    ours.load_state_dict(_seeded_state_dict(sd, rank))
     info = d.compute_distribution_info(P_x, in_shape)
-    theirs_info = ref.compute_distribution_info(P_ref, in_shape)
-    assert tuple(info["shape"]) == tuple(theirs_info["shape"]) and tuple(info["start"]) == tuple(theirs_info["start"])
+    assert tuple(info["shape"]) == tuple(int(s) for s in gold[pre + "shape"])
+    assert tuple(info["start"]) == tuple(int(s) for s in gold[pre + "start"])
     g = torch.Generator().manual_seed(99)
     xg = torch.randn(*in_shape, dtype=torch.float64, generator=g)
     x = xg[tuple(info["slice"])].contiguous()
-    y0, y1 = theirs(x.clone()), ours(x.clone())
+    y1 = ours(x.clone())
+    y0 = torch.from_numpy(gold[pre + "y"])
+    assert y1.shape == y0.shape, (tuple(y1.shape), tuple(y0.shape))
     t = torch.randn(y0.shape, dtype=torch.float64, generator=torch.Generator().manual_seed(5 + rank))
-    l0 = ref.DistributedRelativeLpLoss(P_ref)(y0, t)
     l1 = d.DistributedRelativeLpLoss(P_x)(y1, t)
-    l0.backward()
     l1.backward()
-    g0 = {k: p.grad for k, p in theirs.named_parameters() if p.grad is not None}
+    g0 = {k[len(pre + "grad/"):]: torch.from_numpy(gold[k]) for k in gold.files if k.startswith(pre + "grad/")}
     g1 = {k: p.grad for k, p in ours.named_parameters() if p.grad is not None}
     assert sorted(g0) == sorted(g1)
     gerr = max([float((g0[k] - g1[k]).abs().max()) for k in g0 if g0[k].numel()] or [0.0])
     # off the root the reference's loss is mean(empty / empty) = NaN (it only ever prints the root's value);
     # ours is a well-defined 0 there
-    lerr = abs(float(l0) - float(l1)) if rank == 0 else float(l1)
-    return float((y0 - y1).abs().max()), lerr, gerr
+    lerr = abs(float(gold[pre + "loss"][0]) - float(l1)) if rank == 0 else float(l1)
+    return float((y0 - y1.detach()).abs().max()), lerr, gerr
 
 
 CFG = dict(in_shape=[1, 2, 8, 8, 8, 2], nt=4, width=3, modes=(2, 2, 2, 2), blocks=2)

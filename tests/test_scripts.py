@@ -86,7 +86,8 @@ def test_bench_contract_dry_run():
                        text=True, timeout=300, cwd=ROOT)
     ref = json.loads(r.stdout.strip().splitlines()[-1])
     assert r.returncode == 0 and ref["impl"] == "reference" and ("unavailable" in ref or "value" in ref)
-    impls = ["baseline"] + (["reference"] if os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "dfno")) else [])
+    has_ref = any(os.path.isdir(os.path.join(ROOT, d, "_ref", "dfno")) for d in ("baseline", "oracle"))
+    impls = ["baseline"] + (["reference"] if has_ref else [])
     for impl in impls:
         out = _run(["bench.py", "--gpus", "2", "--impl", impl, *small])
         rec = json.loads([l for l in out.splitlines() if l.startswith("{")][-1])

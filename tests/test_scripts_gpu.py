@@ -1,4 +1,4 @@
-"""The reference's two training scripts on a B200: both must run on the fused sm_100a engine (VERDICT r1:
+"""The reference's two training scripts on a H100: both must run on the fused sm_90a engine (VERDICT r1:
 the Navier-Stokes trainer is 2-D + time, the two-phase default config has T = 30), train, checkpoint, resume and
 -- for the Navier-Stokes script -- draw its curves / GIF."""
 import glob
@@ -35,7 +35,7 @@ def test_navier_stokes_trainer_runs_on_the_fused_engine(tmp_path):
                 "--partition-shape", *grid, "--num-data", "40", "--train-split", "0.75", "--in-timesteps", "10", "--out-timesteps", "40",
                 "--num-epochs", "3", "--batch-size", "10", "--checkpoint-interval", "3", "--generate-visualization",
                 "--out-root", str(tmp_path / "ns")], n)
-    assert "backend = fused sm_100a engine" in log, log[-2000:]
+    assert "backend = fused sm_90a engine" in log, log[-2000:]
     losses = [float(l.split("=")[-1]) for l in log.splitlines() if "average train loss" in l]
     assert len(losses) == 3 and losses[-1] < losses[0], losses
     assert len(glob.glob(str(tmp_path / "ns" / "*" / "model_0003_0000.pt"))) == 1
@@ -50,7 +50,7 @@ def test_two_phase_trainer_default_shape_runs_on_the_fused_engine(tmp_path):
     train = ["training/two_phase/train_two_phase.py", "--num-train", "4", "--num-valid", "1", "--checkpoint-interval", "1",
              "--out-dir", out]
     log = _run(train + ["--epochs", "2"], n)
-    assert "backend = fused sm_100a engine" in log and "training finished." in log, log[-2000:]
+    assert "backend = fused sm_90a engine" in log and "training finished." in log, log[-2000:]
     assert os.path.exists(os.path.join(out, "model_0002_0000.pt"))
     log = _run(train + ["--epochs", "3", "--resume"], n)
     assert "resumed from epoch 2" in log

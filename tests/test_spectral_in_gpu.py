@@ -1,4 +1,4 @@
-"""spectral_in (csrc/spectral_in_sm100.cu): truncated z-DFT -> t-DFT chained through TMEM / shared memory, with the
+"""spectral_in (csrc/spectral_in_sm90.cu): truncated z-DFT -> t-DFT chained through registers / shared memory, with the
 pencil-transpose store, against an fp32 reference of the same two GEMMs (bf16 rounding of Z1 included)."""
 import pytest
 import torch

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Taylor-remainder gradient checks, launchable stand-alone or under torchrun.
 
-Counterparts of the reference's four driver scripts (``/root/reference/tests/gradient_test_torch.py``,
+Counterparts of the reference's four driver scripts (reference ``tests/gradient_test_torch.py``,
 ``gradient_test_distdl.py``, ``gradient_test_distdl_bcast.py``, ``gradient_test_dfno.py``):
 
     python tools/gradient_check.py --case torch

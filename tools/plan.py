@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Print what the fused engine would do for a configuration -- eligibility, per-rank memory by
-category against the 180 GB of a B200, and the GEMM stage chain with its NVLink scatters -- without
+category against the 80 GB of an H100, and the GEMM stage chain with its NVLink scatters -- without
 touching a GPU.
 
     python tools/plan.py --shape 128 128 128 20 --width 20 --modes 12 12 12 10 --gpus 8
@@ -11,7 +11,7 @@ import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from dfno_b200.models.fused import HBM_BUDGET, EnginePlan, supports   # noqa: E402
+from dfno_b200.models.fused import H100_COPY_GBS, HBM_BUDGET, EnginePlan, supports   # noqa: E402
 
 
 class _Grid:
@@ -30,6 +30,9 @@ def main():
     ap.add_argument("--in-channels", type=int, default=1)
     ap.add_argument("--in-timesteps", type=int, default=1)
     ap.add_argument("--blocks", type=int, default=4)
+    ap.add_argument("--hbm-gbs", type=float, default=None,
+                    help="HBM copy bandwidth for the traffic floor (default: the value measured on an H100)")
+    ap.add_argument("--nvlink-gbs", type=float, default=None, help="measured peer-copy rate (default: not estimated)")
     a = ap.parse_args()
     X, Y, Z, T = a.shape
     grid = a.partition or [1, 1, 1, a.gpus, 1, 1]
@@ -53,19 +56,12 @@ def main():
         for k, v in m.items():
             if k != "total" and v:
                 print(f"  {k:22s} {v / 2 ** 30:9.3f} GiB")
-    peaks = {"hbm": 6491.8, "link": 770.0}
-    mp = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")
-    if os.path.exists(mp):
-        try:
-            import json
-            j = json.load(open(mp))
-            peaks["hbm"] = float(j.get("hbm_copy_gbs", j.get("hbm_gbs", peaks["hbm"])))
-        except Exception:       # noqa: BLE001 - fall back to the recorded value
-            pass
+    peaks = {"hbm": a.hbm_gbs or H100_COPY_GBS, "link": a.nvlink_gbs}
     cm = pl.cost_model(hbm_gbs=peaks["hbm"], nvlink_gbs=peaks["link"], front=True)
     print(f"\ntraffic of one training step per rank: {cm['hbm_bytes'] / 1e9:.2f} GB HBM -> {cm['hbm_floor_ms']:.2f} ms at "
-          f"{peaks['hbm']:.0f} GB/s;  {cm['nvlink_bytes'] / 1e6:.0f} MB over NVLink -> {cm['nvlink_ms']:.3f} ms at "
-          f"{peaks['link']:.0f} GB/s (overlappable)")
+          f"{peaks['hbm']:.0f} GB/s;  {cm['nvlink_bytes'] / 1e6:.0f} MB over NVLink" +
+          (f" -> {cm['nvlink_ms']:.3f} ms at {peaks['link']:.0f} GB/s (overlappable)" if peaks["link"] else
+           " (no measured NVLink rate)"))
     for name, calls, hb, lb in cm["stages"]:
         print(f"  {name:18s} x{calls:<3d} {hb / 1e9:8.3f} GB/call" + (f"  + {lb / 1e6:7.1f} MB NVLink" if lb else ""))
     staged = P >= 8

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """2-D Navier-Stokes (space x space x time) FNO experiment -- the workflow of
-``/root/reference/training/navier_stokes/experiment_navier_stokes.py``: the root rank loads and
+reference ``training/navier_stokes/experiment_navier_stokes.py``: the root rank loads and
 normalises the trajectories, the data set is scattered root -> ``P_x`` with a Repartition
 (``:91-93``), training uses Adam(1e-3, wd 1e-4) and the distributed MSE loss, predictions
 are de-normalised before the loss, checkpoints are written per rank, and predictions can
@@ -45,7 +45,7 @@ ap.add_argument("--checkpoint-interval", "-ci", type=int, default=25)
 ap.add_argument("--generate-visualization", "-gv", action="store_true")
 ap.add_argument("--out-root", type=Path, default=Path("data"))
 ap.add_argument("--dtype", default="auto", choices=["auto", "bf16", "fp32"],
-                help="auto: bf16 on a GPU (the fused sm_100a engine serves 2-D + time problems), fp32 on the CPU")
+                help="auto: bf16 on a GPU (the fused sm_90a engine serves 2-D + time problems), fp32 on the CPU")
 args = ap.parse_args()
 
 d.ensure_process_group()
@@ -99,7 +99,7 @@ with ctx:
     net = d.DistributedFNO(P_x, gshape, T_out, args.width, args.modes, num_blocks=args.num_blocks, device=device,
                            dtype=mdtype)
     fused = isinstance(net, d.FusedDistributedFNO)
-    d.print0(f"backend = {'fused sm_100a engine' if fused else 'portable (torch.fft / torch.distributed)'}, dtype = {mdtype}")
+    d.print0(f"backend = {'fused sm_90a engine' if fused else 'portable (torch.fft / torch.distributed)'}, dtype = {mdtype}")
     params = [p for p in net.parameters() if p.numel() > 0]
     criterion, mse = d.DistributedMSELoss(P_x).to(device), d.DistributedMSELoss(P_x).to(device)
     optimizer = (d.FusedAdam(net, lr=1e-3, weight_decay=1e-4) if fused

@@ -2,7 +2,7 @@
 """Inference with a trained two-phase model: rebuild the network, load this rank's
 ``model_{rank:04d}.pt``, predict one validation sample, gather input / truth / prediction onto
 the root with ``Repartition(P_x, P_root)`` and save them
-(``/root/reference/training/two_phase/test_two_phase.py``; the reference's 3-vs-2 input-channel
+(reference ``training/two_phase/test_two_phase.py``; the reference's 3-vs-2 input-channel
 mismatch at ``:69`` is not reproduced)."""
 import argparse
 import os

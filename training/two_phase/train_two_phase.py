@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Two-phase (CO2 plume) FNO training -- the workflow of
-``/root/reference/training/two_phase/train_two_phase.py`` (4-way y-pencil, field 60x60x64x30,
+reference ``training/two_phase/train_two_phase.py`` (4-way y-pencil, field 60x60x64x30,
 width 20, modes (12,12,12,8), 2 input channels, relative-L2 loss, Adam 1e-3, checkpoint every
 10 epochs, loss history on the root) on this framework:
 
@@ -58,7 +58,7 @@ with ctx:
 
     net = d.DistributedFNO(P_x, [nb, 2, *shape[:-1], 1], shape[-1], args.width, args.modes, device=device, dtype=dtype)
     fused = isinstance(net, d.FusedDistributedFNO)
-    d.print0(f"backend = {'fused sm_100a engine' if fused else 'portable (torch.fft / torch.distributed)'}, dtype = {dtype}")
+    d.print0(f"backend = {'fused sm_90a engine' if fused else 'portable (torch.fft / torch.distributed)'}, dtype = {dtype}")
     criterion = d.DistributedRelativeLpLoss(P_x).to(device)
     params = [p for p in net.parameters() if p.numel() > 0]
     optimizer = d.FusedAdam(net, lr=args.lr) if fused else (torch.optim.Adam(params, lr=args.lr) if params else None)
