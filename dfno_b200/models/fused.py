@@ -39,7 +39,7 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from ..ops import operators as OPS
-from ..ops.gemm import ScatterSpec, pad_operator
+from ..ops.gemm import DFT_GEMM_SMEM, ScatterSpec, dft_gemm_fits, dft_gemm_min_smem, pad_operator
 from ..parallel.partition import Partition
 
 __all__ = ["FusedDistributedFNO", "FusedAdam", "supports", "wants", "EnginePlan", "fold_onto_pencil"]
@@ -48,6 +48,7 @@ SUPPORTED_WIDTHS = (4, 8, 12, 16, 20, 24, 32)
 MAX_N = 256                  # n_pad limit of dft_gemm (accumulator columns of one 64-row warpgroup tile)
 HBM_BUDGET = 72 * 2 ** 30    # of an H100's 80 GB: leave room for the CUDA context, NCCL and the allocator
 HEAD_HIDDEN = 128
+LIFT_MAX_W = 4096            # floats of shared memory for the lift weights (kLiftMaxW, csrc/pointwise.cu)
 H100_COPY_GBS = 3027.0       # device-to-device copy bandwidth (GB/s, read + write) measured on an H100 80GB HBM3 at 700 W
 
 
@@ -122,6 +123,10 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
         return False, "Y and 2*modes_z must divide evenly over the pencil"
     if Cin > 4 or Tin > 64:
         return False, "lift kernel covers Cin <= 4 and Tin <= 64"
+    lift_w = T * Tin + T + 2 * (width * Cin + width)
+    if lift_w > LIFT_MAX_W:
+        return False, (f"lift weights need {lift_w} floats of shared memory, more than the lift kernel's "
+                       f"{LIFT_MAX_W} (kLiftMaxW)")
     # T % 4 != 0 (e.g. the reference's two-phase run and in-module demo, T = 30) uses a padded t pitch in Z1
     # (EnginePlan.Tp); covered by tests/test_fused_gpu.py
     if Z % 8 or T % 2 or Y % 4 or (X % 4 and X != 1) or (mx % 2 and X != 1) or my % 2 or mz % 2:
@@ -138,14 +143,22 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
     if need > HBM_BUDGET:
         return False, (f"needs {need / 2 ** 30:.0f} GiB per GPU for training with 4 blocks "
                        f"(budget {HBM_BUDGET / 2 ** 30:.0f} GiB): use more GPUs or a smaller batch")
-    if max(X, Y) > 128:
-        try:                                   # long axes: the inverse stages are issued as column parts
-            for staged in {False, P >= 8}:
-                for st in pl.chain(staged=staged):
-                    if "N" in st:
-                        pl.parts(st)
-        except ValueError as e:
-            return False, str(e)
+    # every GEMM stage keeps its operator (or, for the inverse stages of axes longer than 128 samples, each column
+    # part of it) resident in shared memory; the adjoint chain's operators have the same shapes
+    for staged in {False, P >= 8}:
+        for st in pl.chain(staged=staged):
+            if "N" not in st:
+                continue
+            try:
+                parts = pl.parts(st)
+            except ValueError as e:
+                return False, str(e)
+            for _, n, _, _, _ in parts:
+                rows = 2 * n
+                if not dft_gemm_fits(rows, st["K"]):
+                    return False, (f"stage {st['name']}: a resident {rows} x {st['K']} operator needs "
+                                   f"{dft_gemm_min_smem(rows, st['K']) // 1024} KiB of shared memory, more than "
+                                   f"dft_gemm's {DFT_GEMM_SMEM // 1024} KiB")
     return True, ""
 
 

@@ -7,7 +7,7 @@ import torch
 
 from . import build
 
-__all__ = ["pad_operator", "gemm_rowmajor", "gemm_scatter", "ScatterSpec"]
+__all__ = ["pad_operator", "dft_gemm_min_smem", "dft_gemm_fits", "gemm_rowmajor", "gemm_scatter", "ScatterSpec"]
 
 EPI_ROWMAJOR, EPI_PAIR_SCATTER = 0, 1
 PEER_NONE, PEER_BY_ROW, PEER_BY_COL = 0, 1, 2
@@ -23,6 +23,26 @@ def pad_operator(B: torch.Tensor, device=None) -> torch.Tensor:
     out = torch.zeros(_ceil(N, 16), _ceil(K, 64), dtype=torch.bfloat16, device=device or B.device)
     out[:N, :K] = B.to(device=out.device, dtype=torch.bfloat16)
     return out
+
+
+# Shared-memory sizing of dft_gemm_launch (csrc/dft_gemm_sm90.cu); keep the two in step.  The padded operator stays
+# resident next to 5 KB of barriers, tables and alignment slack, the row scratch of one consumer warpgroup
+# (4 warps x kRowScratchFloats = 32 x 17 floats) and a ring of at least two A stages of one 64-wide K block each
+# (64 rows when n_pad > 128, else 128).  Any other configuration the launcher tries needs more.
+DFT_GEMM_SMEM = 227 * 1024
+
+
+def dft_gemm_min_smem(rows: int, cols: int) -> int:
+    """Fewest bytes of shared memory ``dft_gemm`` needs with a resident ``[rows, cols]`` operator."""
+    n_pad, k_pad = _ceil(rows, 16), _ceil(cols, 64)
+    tile_m = 64 if n_pad > 128 else 128
+    return n_pad * k_pad * 2 + 4096 + 1024 + 4 * 32 * 17 * 4 + 2 * tile_m * 64 * 2
+
+
+def dft_gemm_fits(rows: int, cols: int) -> bool:
+    """Can ``dft_gemm`` keep a ``[rows, cols]`` operator resident (padded to ``[ceil16(rows), ceil64(cols)]``)?"""
+    return (_ceil(rows, 16) <= 256 and _ceil(cols, 64) <= 512
+            and dft_gemm_min_smem(rows, cols) <= DFT_GEMM_SMEM)
 
 
 def gemm_rowmajor(A: torch.Tensor, M: int, K: int, lda: int, Bpad: torch.Tensor, N: int,

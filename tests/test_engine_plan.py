@@ -208,6 +208,60 @@ def test_supports_covers_the_baseline_configs():
     assert not supports(_Grid(1, 1, 1, 1, 1, 1), [1, 1, 512, 64, 64, 1], 16, 20, (8, 8, 8, 8))[0]     # X > 256
 
 
+def test_supports_refuses_lift_weights_over_the_kernel_budget():
+    """The lift kernel keeps W1, b1 and the packed W2, b2 in 4096 floats of shared memory (kLiftMaxW)."""
+    from dfno_b200.models.fused import LIFT_MAX_W, supports, wants
+    g = _Grid(1, 1, 1, 1, 1, 1)
+    assert 62 * 64 + 62 + 2 * (8 + 8) <= LIFT_MAX_W < 64 * 64 + 64 + 2 * (8 + 8)
+    assert supports(g, [1, 1, 8, 8, 16, 64], 62, 8, (2, 2, 4, 4))[0]
+    ok, why = supports(g, [1, 1, 8, 8, 16, 64], 64, 8, (2, 2, 4, 4))
+    assert not ok and "4192" in why and "kLiftMaxW" in why, why
+    kw = dict(device=torch.device("cuda"), dtype=torch.bfloat16)
+    assert not wants((g, [1, 1, 8, 8, 16, 64], 64, 8, (2, 2, 4, 4)), kw, "auto")
+    assert wants((g, [1, 1, 8, 8, 16, 64], 62, 8, (2, 2, 4, 4)), kw, "auto")
+    with pytest.raises(ValueError, match="kLiftMaxW"):
+        wants((g, [1, 1, 8, 8, 16, 64], 64, 8, (2, 2, 4, 4)), kw, "fused")
+
+
+def test_dft_gemm_sizing_mirrors_the_launcher():
+    """dft_gemm_min_smem: operator + 5 KB fixed + 8.5 KB row scratch of one warpgroup + two A stages of one K block
+    (8 KB each with 64-row tiles, n_pad > 128; 16 KB with 128-row tiles), within 227 KB."""
+    from dfno_b200.ops.gemm import DFT_GEMM_SMEM, dft_gemm_fits, dft_gemm_min_smem
+    assert DFT_GEMM_SMEM == 227 * 1024
+    assert dft_gemm_min_smem(192, 512) == 192 * 512 * 2 + 5120 + 8704 + 2 * 8192
+    assert dft_gemm_min_smem(128, 512) == 128 * 512 * 2 + 5120 + 8704 + 2 * 16384
+    assert dft_gemm_min_smem(190, 500) == dft_gemm_min_smem(192, 512)          # padded to [ceil16, ceil64]
+    assert dft_gemm_fits(192, 512) and not dft_gemm_fits(200, 512) and not dft_gemm_fits(208, 512)
+    assert dft_gemm_fits(256, 256) and not dft_gemm_fits(256, 400)
+    assert not dft_gemm_fits(272, 64) and not dft_gemm_fits(16, 576)           # the launcher's n_pad / k_pad limits
+    # the stage shapes the check uses are those of the operators the engine pads
+    pl = EnginePlan(1, 1, 1, 8, 20, 256, 256, 64, (8, 40, 12, 10))
+    pl.finish(1)
+    ops = pl.operators()
+    for st in pl.chain():
+        if "N" in st:
+            assert tuple(ops[st["op"]].shape) == (st["N"], st["K"]) == tuple(ops[st["op"] + "_adj"].shape), st["name"]
+
+
+@pytest.mark.parametrize("in_shape,modes,accept,stage", [
+    ([1, 1, 4, 256, 8, 1], (2, 48, 2, 2), True, None),      # G2 / G2_adj: 192 x 512 bf16 (n_pad 192) fits
+    ([1, 1, 4, 256, 8, 1], (2, 50, 2, 2), False, "G2"),     # n_pad 208: 237 KiB
+    ([1, 1, 4, 256, 8, 1], (2, 64, 2, 2), False, "G2"),     # 256 x 512 bf16 = 256 KB
+    ([1, 1, 256, 4, 8, 1], (48, 2, 2, 2), True, None),      # the same on the x axis (G3)
+    ([1, 1, 256, 4, 8, 1], (52, 2, 2, 2), False, "G3"),
+    ([1, 1, 8, 8, 256, 1], (2, 2, 100, 2), False, "iG1a"),  # legacy pointwise route: iG1a is 256 x 400
+])
+def test_supports_refuses_operators_too_large_for_shared_memory(in_shape, modes, accept, stage):
+    from dfno_b200.models.fused import supports, wants
+    g = _Grid(1, 1, 1, 1, 1, 1)
+    ok, why = supports(g, in_shape, 4, 4, modes)
+    assert ok == accept, why
+    if not accept:
+        assert f"stage {stage}:" in why and "shared memory" in why, why
+    kw = dict(device=torch.device("cuda"), dtype=torch.bfloat16)
+    assert wants((g, in_shape, 4, 4, modes), kw, "auto") == accept
+
+
 def test_memory_plan_sizes_shards_for_a_b200():
     from dfno_b200.models.fused import HBM_BUDGET, supports
     pl = EnginePlan(1, 1, 1, 20, 20, 128, 128, 128, (12, 12, 12, 10), world=1, rank=0)

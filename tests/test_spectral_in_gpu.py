@@ -23,7 +23,7 @@ def _reference(h, o1, o2, BC, X, Yl, T, Z, KZ, mt):
 
 @pytest.mark.parametrize("BC,X,Yl,T,Z,mz,mt,P", [
     (6, 5, 32, 20, 128, 12, 10, 1),       # the headline tile: Rp = 4, Yc = 32
-    (8, 16, 128, 20, 128, 12, 10, 1),     # 512 chunks on 148 CTAs: several chunks per CTA, both staging buffers
+    (8, 16, 128, 20, 128, 12, 10, 1),     # 512 chunks on 132 CTAs (H100 SXM): several chunks per CTA, both staging buffers
     (8, 64, 256, 4, 8, 2, 2, 1),          # tiny tiles (T = 4, Z = 8), 32 tiles per CTA: the issuing warps run far ahead of the epilogue
     (4, 3, 12, 30, 64, 12, 8, 1),         # T = 30 (two-phase), Yl < Yc = 16: the store is clipped at the row end
     (4, 1, 16, 32, 256, 16, 8, 1),        # 2-D + time (X = 1), Z = 256: four K blocks
