@@ -74,16 +74,27 @@ struct HeadFwdParams {
   RowMap map;
 };
 
+// The epilogue works on the accumulator fragment: thread (warp q of the warpgroup, lane l) holds 4 positions of the
+// tile (frag_row) and, for each, the 32 hidden units 8j + 2(l%4) + {0, 1}; the W4 dot is finished across the 4
+// lanes of a quad.
+__device__ __forceinline__ int frag_row(int q, int lane, int k) {     // k = 0..3: the thread's rows of a 128-row tile
+  return 64 * (k >> 1) + 16 * q + (lane >> 2) + 8 * (k & 1);
+}
+__device__ __forceinline__ float pick4(const float (&v)[4], int k) {   // v[k] for a run-time k, without local memory
+  return k == 0 ? v[0] : k == 1 ? v[1] : k == 2 ? v[2] : v[3];
+}
+
+// KR: channels + the ones row, padded to 16 (the K of the MMA)
+template <int KR>
 __global__ void __launch_bounds__(kThreadsHF, 1)
 head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
                 const HeadFwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* s_w3 = smem;                                    // [128 hid][64] K-major, column C = b3
   uint8_t* s_a = smem + 16384;                             // stages x 2 halves x [KR rows][64 pos]
-  const uint32_t half_bytes = static_cast<uint32_t>(p.KR) * 128;
-  const uint32_t stage_bytes = 2 * half_bytes;
-  float* s_scratch = reinterpret_cast<float*>(s_a + kStagesHF * stage_bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_scratch + 4 * kGroupsHF * kRowScratchFloats);
+  constexpr uint32_t half_bytes = KR * 128;
+  constexpr uint32_t stage_bytes = 2 * half_bytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_a + kStagesHF * stage_bytes);
   uint64_t* full = bars;              // [6]
   uint64_t* empty = bars + 6;         // [6]
   uint64_t* wfull = bars + 12;
@@ -130,12 +141,13 @@ head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__
     }
     return;
   }
-  const int q = warp & 3, g = warp >> 2;
-  const int m = wg_row128(q, lane);
-  float* scratch = s_scratch + warp * kRowScratchFloats;
+  const int q = warp & 3, g = warp >> 2, cq = lane & 3;
+  const int my_row = frag_row(q, lane, cq);          // the row this lane stores (each lane of a quad stores one)
   const float b4 = s_b4[0];
-  const int ksteps = p.KR >> 4;
   const uint32_t w_addr = smem_u32(s_w3);
+  uint32_t w4[16];                                   // W4 pairs of this thread's hidden units 8j + 2(l%4) + {0, 1}
+#pragma unroll
+  for (int j = 0; j < 16; ++j) w4[j] = s_w4[4 * j + cq];
   mbar_wait(wfull, 0);
   float acc[128];
   long long n = 0;
@@ -143,41 +155,52 @@ head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__
     if (n % kGroupsHF != g) continue;
     const uint32_t s = static_cast<uint32_t>(n % kStagesHF);
     const int b = static_cast<int>(tile / p.tiles_per_b);
-    const long long pos = (tile % p.tiles_per_b) * 128 + m;
+    const long long pos = (tile % p.tiles_per_b) * 128 + my_row;
     mbar_wait(&full[s], (n / kStagesHF) & 1);
     // pre[pos, j] = sum_c h[c, pos] W3aug[j, c]: A MN-major (positions contiguous, 64-position halves half_bytes apart)
     const uint32_t abase = smem_u32(s_a + s * stage_bytes);
     wgmma_fence();
-    for (int ks = 0; ks < ksteps; ++ks)
+#pragma unroll
+    for (int ks = 0; ks < KR / 16; ++ks)
       wg_mma128<false, 1, 0>(acc, kHidH, gdesc_mn128(abase + ks * 2048, half_bytes, 1024), half_bytes,
                              gdesc_k128(w_addr + ks * 32), ks > 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
     acc_fence(acc);
     if (q == 0 && lane == 0) mbar_arrive(&empty[s]);
-    float out = b4;
+    // row k of the thread: registers 64(k/2) + 4j + 2(k%2) + {0, 1}; two fp16 dot chains of 8 pairs each
+    float out[4];
 #pragma unroll
-    for (int ch = 0; ch < 8; ++ch) {
-      uint32_t v[16];
-      wg_row16<2>(acc, ch * 16, scratch, v);
-      const uint4 wa = reinterpret_cast<const uint4*>(s_w4)[2 * ch], wb = reinterpret_cast<const uint4*>(s_w4)[2 * ch + 1];
-      const uint32_t w[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w};
-      __half2 part = __float2half2_rn(0.f);
+    for (int k = 0; k < 4; ++k) {
+      const float* a = acc + 64 * (k >> 1) + 2 * (k & 1);
+      float sum = 0.f;
 #pragma unroll
-      for (int i = 0; i < 8; ++i)
-        part = __hfma2(gelu_h2(h2_from_f32(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]))),
-                       h2_of_bits(w[i]), part);
-      const float2 f = __half22float2(part);
-      out += f.x + f.y;
+      for (int half = 0; half < 2; ++half) {
+        __half2 part = __float2half2_rn(0.f);
+#pragma unroll
+        for (int j = 8 * half; j < 8 * half + 8; ++j)
+          part = __hfma2(gelu_h2(h2_from_f32(a[4 * j], a[4 * j + 1])), h2_of_bits(w4[j]), part);
+        const float2 f = __half22float2(part);
+        sum += f.x + f.y;
+      }
+      sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+      sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+      out[k] = sum;
     }
-    if (pos < p.S) p.out[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] = out;
+    if (pos < p.S) p.out[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] = b4 + pick4(out, cq);
   }
 }
 
 // ================================================================================ backward
 constexpr int kMaxStagesHB = 6;                 // h tiles are small: deep prefetch keeps TMA latency off the consumers
 constexpr int kGroupsHB = 2;                    // consumer warpgroups (stages a multiple of it: see bypass_sm90.cu)
-constexpr int kThreadsHB = 128 * kGroupsHB + 32;
+// One producer WARPGROUP (one warp issues TMA): setmaxnreg moves its registers to the consumers, whose fragment
+// epilogues need more than the uniform 168 per thread of a 384-thread block.
+constexpr int kThreadsHB = 128 * kGroupsHB + 128;
+constexpr int kProducerRegsHB = 24, kConsumerRegsHB = 240;
+static_assert(128 * kProducerRegsHB + 128 * kGroupsHB * kConsumerRegsHB <= 65536, "register file");
+template <int KR>
+constexpr bool kWsumSmem = KR > 32;
 
 struct HeadBwdParams {
   int B, C, KR, stages;
@@ -185,28 +208,33 @@ struct HeadBwdParams {
   const float* dout;          // fp32, public layout
   const float* amax;          // max |dout| (device scalar)
   const float* W4;
-  __nv_bfloat16* g;           // [B*C, S]
   float* gW3; float* gb3; float* gW4; float* gb4;
   RowMap map;
 };
 
 // Per tile of 128 positions, one consumer warpgroup runs the backward of the file header; MMA1 in two
-// 64-column halves so that the D3 accumulator fits next to it.
+// 64-column halves so that the D3 accumulator fits next to it.  Both epilogues work on the accumulator fragments
+// (frag_row): epilogue A turns each MMA1 half into P in registers, which feeds MMA2 as its register A operand and is
+// stored once with stmatrix for MMA3; dW4 stays in per-thread column registers until the flush; epilogue B stages
+// g as bf16 [C][128 positions] with stmatrix.trans and writes it with two TMA stores.
 // KR: channels + the ones row, padded to 16 (the N of MMA2 / MMA3 and the accumulator width)
 template <int KR>
 __global__ void __launch_bounds__(kThreadsHB, 1)
 head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
-                 const __grid_constant__ CUtensorMap tmW3T, const HeadBwdParams p) {
+                 const __grid_constant__ CUtensorMap tmW3T, const __grid_constant__ CUtensorMap tmG,
+                 const HeadBwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t half_bytes = static_cast<uint32_t>(KR) * 128;
-  const uint32_t tile_bytes = 2 * half_bytes;
+  constexpr uint32_t half_bytes = KR * 128;
+  constexpr uint32_t tile_bytes = 2 * half_bytes;
   uint8_t* s_w3 = smem;                                   // 16 KB
   uint8_t* s_w3t = s_w3 + 16384;                          // 2 k-blocks x [KR c rows][64 hid] fp16
   uint8_t* s_p = s_w3t + tile_bytes;                      // per warpgroup: 2 x [128 pos][64 hid] fp16
   uint8_t* s_a = s_p + kGroupsHB * 32768;                 // stages x h tile
   uint8_t* s_hs = s_a + p.stages * tile_bytes;            // per warpgroup: scaled fp16 copy of the h tile
-  float* s_scratch = reinterpret_cast<float*>(s_hs + kGroupsHB * tile_bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_scratch + 4 * kGroupsHB * kRowScratchFloats);
+  uint8_t* s_g = s_hs + kGroupsHB * tile_bytes;           // per warpgroup: bf16 g staging, 2 x [KR c rows][64 pos]
+  // KR = 48 leaves no registers for the dW4 column sums: they live in [32][consumer threads] floats instead
+  float* s_wsum = reinterpret_cast<float*>(s_g + kGroupsHB * tile_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_wsum + (kWsumSmem<KR> ? 32 * 128 * kGroupsHB : 0));
   uint64_t* a_full = bars;            // [8]
   uint64_t* a_empty = bars + 8;       // [8]
   uint64_t* w_full = bars + 16;
@@ -230,7 +258,7 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
   for (int i = threadIdx.x; i < 64; i += blockDim.x) s_w4h[i] = h2_bits(h2_from_f32(p.W4[2 * i], p.W4[2 * i + 1]));
   for (int i = threadIdx.x; i < kHidH; i += blockDim.x) s_gw4[i] = 0.f;
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmH); tma_prefetch_desc(&tmW3); tma_prefetch_desc(&tmW3T);
+    tma_prefetch_desc(&tmH); tma_prefetch_desc(&tmW3); tma_prefetch_desc(&tmW3T); tma_prefetch_desc(&tmG);
     for (int s = 0; s < p.stages; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
     mbar_init(w_full, 1);
     fence_barrier_init();
@@ -240,8 +268,9 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
   const float amax = *p.amax;
   const float scale = amax > 0.f ? exp2f(-ceilf(log2f(amax))) : 1.0f;      // |scale * dout| <= 1
 
-  if (warp == 4 * kGroupsHB) {
-    if (lane == 0) {
+  if (warp >= 4 * kGroupsHB) {
+    setmaxnreg_dec<kProducerRegsHB>();
+    if (warp == 4 * kGroupsHB && lane == 0) {
       mbar_arrive_expect_tx(w_full, 16384 + tile_bytes);
       tma_load_2d(s_w3, &tmW3, w_full, 0, 0);
       tma_load_2d(s_w3t, &tmW3T, w_full, 0, 0);
@@ -261,92 +290,129 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
     return;
   }
 
-  const int q = warp & 3, g = warp >> 2;
-  const int m = wg_row128(q, lane);                  // position inside the tile
-  float* scratch = s_scratch + warp * kRowScratchFloats;
+  setmaxnreg_inc<kConsumerRegsHB>();
+  const int q = warp & 3, g = warp >> 2, cq = lane & 3;
+  const int my_row = frag_row(q, lane, cq);          // the row whose dout this lane loads
   const uint32_t barid = 1 + g;
-  const int k1steps = KR >> 4;
+  const bool leader = q == 0 && lane == 0;           // releases ring stages and issues this warpgroup's g stores
   uint8_t* pbuf = s_p + g * 32768;
   uint8_t* hsbuf = s_hs + g * tile_bytes;
+  uint8_t* gbuf = s_g + g * tile_bytes;
   const uint32_t w3_addr = smem_u32(s_w3), w3t_addr = smem_u32(s_w3t);
-  const uint32_t p_addr = smem_u32(pbuf), hs_addr = smem_u32(hsbuf);
+  const uint32_t p_addr = smem_u32(pbuf), hs_addr = smem_u32(hsbuf), g_addr = smem_u32(gbuf);
+  // stmatrix: lane 8i + k addresses row k of matrix i.  P (epilogue A): matrix i = positions 16q + 8(i%2) + k of an
+  // m64 half, hidden units 8(i/2).. of a k16 step.  g (epilogue B, transposed): memory row k of matrix i = channel
+  // 8(i/2) + k of a 16-channel group, holding positions 16q + 8(i%2) .. + 7 (16-byte chunk 2q + i%2 of the row).
+  const int mi = lane >> 3, mk = lane & 7;
+  const uint32_t p_row = 16 * q + 8 * (mi & 1) + mk;
+  const uint32_t g_chunk = 2 * q + (mi & 1);
   float acc_gb4 = 0.f;
+  float wsum[32];                                    // [16 hh + 2 j + e]: dW4 of hidden unit 64 hh + 8 j + 2(l%4) + e
+  float* my_wsum = s_wsum + (threadIdx.x & (128 * kGroupsHB - 1));   // its shared slots (stride 128 kGroupsHB)
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    if constexpr (kWsumSmem<KR>) my_wsum[i * 128 * kGroupsHB] = 0.f;
+    else wsum[i] = 0.f;
+  }
+  // dW4 column sum i += v
+  auto wsum_add = [&](int i, float d, float v) {
+    if constexpr (kWsumSmem<KR>) my_wsum[i * 128 * kGroupsHB] = fmaf(d, v, my_wsum[i * 128 * kGroupsHB]);
+    else wsum[i] = fmaf(d, v, wsum[i]);
+  };
   float d3[KR];                                      // [hid, c] over this warpgroup's tiles: 128 x KR
+  uint32_t pa[2][4][4];                              // P of one 64-unit hidden half: [m64 half][k16 step][A register]
+  // MMA2, hidden units [64 kb, 64 kb + 64): dh0 (+)= P . W3, A = the P registers
+  auto mma2 = [&](float (&acc2)[KR], int kb) {
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      const uint64_t db = gdesc_k128(w3t_addr + kb * half_bytes + ks * 32);
+      const uint32_t sc = (kb > 0 || ks > 0) ? 1u : 0u;
+      wg_mma64_rs<KR, 0, 0>(acc2, pa[0][ks], db, sc);
+      wg_mma64_rs<KR, 0, KR / 2>(acc2, pa[1][ks], db, sc);
+    }
+  };
   long long n = 0, mine = 0;
   mbar_wait(w_full, 0);
   for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
     if (n % kGroupsHB != g) continue;
     const uint32_t s = static_cast<uint32_t>(n % p.stages);
     const int b = static_cast<int>(tile / p.tiles_per_b);
-    const long long pos = (tile % p.tiles_per_b) * 128 + m;
-    const float dout = pos < p.S ? p.dout[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] : 0.f;
-    acc_gb4 += dout;
+    const long long p0 = (tile % p.tiles_per_b) * 128;
+    const long long pos = p0 + my_row;
+    const float dl = pos < p.S ? p.dout[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] : 0.f;
+    acc_gb4 += dl;
+    float dk[4];                                     // dout of the thread's rows frag_row(q, lane, k)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) dk[k] = __shfl_sync(0xffffffffu, dl, (lane & ~3) | k);
     mbar_wait(&a_full[s], (n / p.stages) & 1);
     const uint32_t abase = smem_u32(s_a + s * tile_bytes);
-    uint8_t* prow = pbuf + m * 128;
+    float acc2[KR];                                  // dh0 [pos, c]: 128 x KR
 #pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {                         // hidden units [64 hh, 64 hh + 64)
+    for (int hh = 0; hh < 2; ++hh) {                 // hidden units [64 hh, 64 hh + 64)
       float acc[64];
       wgmma_fence();
-      for (int ks = 0; ks < k1steps; ++ks)
+#pragma unroll
+      for (int ks = 0; ks < KR / 16; ++ks)
         wg_mma128<false, 1, 0>(acc, 64, gdesc_mn128(abase + ks * 2048, half_bytes, 1024), half_bytes,
                                gdesc_k128(w3_addr + hh * 8192 + ks * 32), ks > 0 ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<0>();
       acc_fence(acc);
+      // ---- epi A: P = W4 gelu'(pre) into the A registers and the smem tile; dW4 += dout gelu(pre)
 #pragma unroll
-      for (int ch = 0; ch < 4; ++ch) {                       // 16 hidden units per chunk
-        uint32_t v[16];
-        wg_row16<2>(acc, ch * 16, scratch, v);
-        const uint4 w4 = reinterpret_cast<const uint4*>(s_w4h + 32 * hh + 8 * ch)[0];
-        const uint4 w4b = reinterpret_cast<const uint4*>(s_w4h + 32 * hh + 8 * ch)[1];
-        const uint32_t ww[8] = {w4.x, w4.y, w4.z, w4.w, w4b.x, w4b.y, w4b.z, w4b.w};
-        uint32_t pw[8];
-        float wsum[16];
+      for (int mh = 0; mh < 2; ++mh) {
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const GeluH2 vg = gelu_vg_h2(h2_from_f32(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1])));
-          pw[i] = h2_bits(__hmul2(vg.grad, h2_of_bits(ww[i])));
-          const float2 a = __half22float2(vg.value);
-          wsum[2 * i] = dout * a.x;
-          wsum[2 * i + 1] = dout * a.y;
+        for (int ks = 0; ks < 4; ++ks) {
+          afrag_from_acc(acc + 32 * mh, ks, pa[mh][ks], [&](float lo, float hi, int i) {
+            const int j = 2 * ks + (i >> 1);
+            const GeluH2 vg = gelu_vg_h2(h2_from_f32(lo, hi));
+            const float2 a = __half22float2(vg.value);
+            const float d = dk[2 * mh + (i & 1)];
+            wsum_add(16 * hh + 2 * j, d, a.x);
+            wsum_add(16 * hh + 2 * j + 1, d, a.y);
+            return h2_bits(__hmul2(vg.grad, h2_of_bits(s_w4h[32 * hh + 4 * j + cq])));
+          });
+          const uint32_t row = 64 * mh + p_row, chunk = 2 * ks + (mi >> 1);
+          stmatrix_x4(p_addr + hh * 16384 + row * 128 + ((chunk ^ (row & 7)) << 4), pa[mh][ks]);
         }
-        const uint32_t chunk = 2 * ch;                       // 16-byte chunks of this row in the 64-wide hid block
-        uint8_t* blk = prow + hh * 16384;
-        *reinterpret_cast<uint4*>(blk + ((chunk ^ (m & 7)) << 4)) = make_uint4(pw[0], pw[1], pw[2], pw[3]);
-        *reinterpret_cast<uint4*>(blk + (((chunk + 1) ^ (m & 7)) << 4)) = make_uint4(pw[4], pw[5], pw[6], pw[7]);
-        const float sw = warp_transpose_reduce16(wsum, lane);
-        if (lane < 16) atomicAdd(&s_gw4[64 * hh + 16 * ch + lane], sw);
+      }
+      if (hh == 0) {                                 // MMA2 over the first half, before the second half's MMA1
+        wgmma_fence();
+        mma2(acc2, 0);
+        wgmma_commit();
+        wgmma_wait<0>();
       }
     }
     {
-      // ---- hs: scaled fp16 copy of this position's column; row C = the scaled gradient itself
-      const float ds = dout * scale;
-      const uint32_t colo = (m >> 6) * half_bytes + ((m & 7) << 1);
-      const uint32_t ch = (m & 63) >> 3;
+      // ---- hs: scaled fp16 copy of the h tile at the thread's rows, channels c = l%4 (mod 4); row C = the scaled
+      // gradient itself
       const uint8_t* src = s_a + s * tile_bytes;
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        if (c < p.C) {
+      for (int k = 0; k < 4; ++k) {
+        const int row = frag_row(q, lane, k);
+        const float ds = dk[k] * scale;
+        const uint32_t colo = (row >> 6) * half_bytes + ((row & 7) << 1);
+        const uint32_t ch = (row & 63) >> 3;
+#pragma unroll
+        for (int cc = 0; cc < KR / 4; ++cc) {
+          const int c = 4 * cc + cq;
           const uint32_t off = colo + c * 128 + ((ch ^ (c & 7)) << 4);
-          const uint16_t hv = *reinterpret_cast<const uint16_t*>(src + off);
-          *reinterpret_cast<__half*>(hsbuf + off) = __float2half_rn(__uint_as_float(static_cast<uint32_t>(hv) << 16) * ds);
+          if (c < p.C) {
+            const uint16_t hv = *reinterpret_cast<const uint16_t*>(src + off);
+            *reinterpret_cast<__half*>(hsbuf + off) = __float2half_rn(__uint_as_float(static_cast<uint32_t>(hv) << 16) * ds);
+          } else if (c == p.C) {
+            *reinterpret_cast<__half*>(hsbuf + off) = __float2half_rn(ds);
+          }
         }
       }
-      *reinterpret_cast<__half*>(hsbuf + colo + p.C * 128 + ((ch ^ (p.C & 7)) << 4)) = __float2half_rn(ds);
     }
+    if (leader) tma_store_wait_read();               // the previous tile's g staging is free after the barrier
     fence_proxy_async_smem();
     asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
-    float acc2[KR];                                          // dh0 [pos, c]: 128 x KR
     wgmma_fence();
+    mma2(acc2, 1);
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {                         // K = hid
-      const uint32_t kb = ks >> 2, kk = ks & 3;
-      wg_mma128<true, 0, 0>(acc2, KR, gdesc_k128(p_addr + kb * 16384 + kk * 32), 8192,
-                            gdesc_k128(w3t_addr + kb * half_bytes + kk * 32), ks > 0 ? 1u : 0u);
-    }
-#pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {                         // K = positions; A = P read MN-major (hid contiguous)
+    for (int ks = 0; ks < 8; ++ks) {                 // K = positions; A = P read MN-major (hid contiguous)
       const uint32_t kb = ks >> 2, kk = ks & 3;
       wg_mma128<true, 1, 0>(d3, KR, gdesc_mn128(p_addr + ks * 2048, 16384, 1024), 16384,
                             gdesc_k128(hs_addr + kb * half_bytes + kk * 32), (mine > 0 || ks > 0) ? 1u : 0u);
@@ -356,22 +422,33 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
     acc_fence(acc2);
     acc_fence(d3);
     ++mine;
-    if (q == 0 && lane == 0) mbar_arrive(&a_empty[s]);
-    // ---- epi B: g[c, pos] = dout * dh0[pos, c]
+    if (leader) mbar_arrive(&a_empty[s]);
+    // ---- epi B: g[c, pos] = dout * dh0[pos, c], staged as bf16 [c][64 pos] x 2 (the TMA box layout)
 #pragma unroll
-    for (int cb = 0; cb < KR / 16; ++cb) {
-      {
-        uint32_t v[16];
-        wg_row16<2>(acc2, cb * 16, scratch, v);
-        if (pos < p.S) {
-          __nv_bfloat16* gp = p.g + (static_cast<long long>(b) * p.C + 16 * cb) * p.S + pos;
+    for (int mh = 0; mh < 2; ++mh) {
 #pragma unroll
-          for (int i = 0; i < 16; ++i)
-            if (16 * cb + i < p.C) gp[static_cast<long long>(i) * p.S] = __float2bfloat16(dout * __uint_as_float(v[i]));
+      for (int t = 0; t < KR / 16; ++t) {
+        uint32_t r[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float* a = acc2 + (KR / 2) * mh + 4 * (2 * t + (i >> 1)) + 2 * (i & 1);
+          const float d = dk[2 * mh + (i & 1)];
+          r[i] = pack_bf16x2(d * a[0], d * a[1]);
         }
+        const uint32_t c = 16 * t + 8 * (mi >> 1) + mk;
+        stmatrix_x4_trans(g_addr + mh * half_bytes + c * 128 + ((g_chunk ^ (c & 7)) << 4), r);
       }
     }
+    fence_proxy_async_smem();
+    asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
+    if (leader) {
+      const int row0 = b * p.C;
+      tma_store_2d(&tmG, gbuf, static_cast<int32_t>(p0), row0);
+      if (p0 + 64 < p.S) tma_store_2d(&tmG, gbuf + half_bytes, static_cast<int32_t>(p0 + 64), row0);
+      tma_store_commit();
+    }
   }
+  if (leader) tma_store_wait_all();
   // ---- per-CTA flush of the weight gradients
   acc_gb4 += __shfl_xor_sync(0xffffffffu, acc_gb4, 16);
   acc_gb4 += __shfl_xor_sync(0xffffffffu, acc_gb4, 8);
@@ -379,6 +456,14 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
   acc_gb4 += __shfl_xor_sync(0xffffffffu, acc_gb4, 2);
   acc_gb4 += __shfl_xor_sync(0xffffffffu, acc_gb4, 1);
   if (lane == 0) atomicAdd(s_gb4, acc_gb4);
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {                     // lanes with equal l%4 hold the same hidden units
+    float v = kWsumSmem<KR> ? my_wsum[i * 128 * kGroupsHB] : wsum[i];
+    v += __shfl_xor_sync(0xffffffffu, v, 4);
+    v += __shfl_xor_sync(0xffffffffu, v, 8);
+    v += __shfl_xor_sync(0xffffffffu, v, 16);
+    if (lane < 4) atomicAdd(&s_gw4[64 * (i >> 4) + 8 * ((i & 15) >> 1) + 2 * cq + (i & 1)], v);
+  }
   if (mine > 0) {
     // fragment of the 128 x KR accumulator: register (KR/2)h + 4j + e holds hidden unit 64h + 16q + lane/4 + 8(e/2),
     // column 8j + 2(lane%4) + e%2
@@ -443,16 +528,22 @@ const char* head_fwd(const void* h, const void* W3aug, const float* w4b4, float*
   CUtensorMap tmH, tmW3;
   if (make_map_2d(&tmH, h, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (h) failed";
   if (make_map_2d(&tmW3, W3aug, 64, 128, 64, 64, 128)) return "tensor map (W3) failed";
-  static bool attr = false;
-  if (!attr) {
-    if (cudaFuncSetAttribute(head_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+  static bool attr[3] = {false, false, false};
+  const int kr_i = p.KR / 16 - 1;
+  const void* fn = kr_i == 0 ? reinterpret_cast<const void*>(head_fwd_kernel<16>)
+                 : kr_i == 1 ? reinterpret_cast<const void*>(head_fwd_kernel<32>)
+                             : reinterpret_cast<const void*>(head_fwd_kernel<48>);
+  if (!attr[kr_i]) {
+    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
       return "cudaFuncSetAttribute failed";
-    attr = true;
+    attr[kr_i] = true;
   }
-  const uint32_t smem_bytes = 16384 + kStagesHF * 2 * p.KR * 128 + 4 * kGroupsHF * kRowScratchFloats * 4 + 2048 + 1024;
+  const uint32_t smem_bytes = 16384 + kStagesHF * 2 * p.KR * 128 + 2048 + 1024;
   const long long tiles = p.tiles_per_b * B;
   const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
-  head_fwd_kernel<<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
+  if (kr_i == 0) head_fwd_kernel<16><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
+  else if (kr_i == 1) head_fwd_kernel<32><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
+  else head_fwd_kernel<48><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
@@ -468,12 +559,13 @@ const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const
   HeadBwdParams p{};
   p.B = B; p.C = C; p.KR = (C + 1 + 15) / 16 * 16; p.S = S; p.tiles_per_b = (S + 127) / 128;
   p.dout = dout; p.amax = reinterpret_cast<const float*>(amax_ws); p.W4 = W4;
-  p.g = static_cast<__nv_bfloat16*>(g); p.gW3 = gW3; p.gb3 = gb3; p.gW4 = gW4; p.gb4 = gb4;
+  p.gW3 = gW3; p.gb3 = gb3; p.gW4 = gW4; p.gb4 = gb4;
   if (set_rowmap(&p.map, nrl, R, SR)) return "head_bwd: 1..4 row digits";
-  CUtensorMap tmH, tmW3, tmW3T;
+  CUtensorMap tmH, tmW3, tmW3T, tmG;
   if (make_map_2d(&tmH, h, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (h) failed";
   if (make_map_2d(&tmW3, W3aug, 64, 128, 64, 64, 128)) return "tensor map (W3) failed";
   if (make_map_2d(&tmW3T, W3T16, 128, p.KR, 128, 64, p.KR)) return "tensor map (W3T) failed";
+  if (make_map_2d(&tmG, g, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (g) failed";
   static bool attr[3] = {false, false, false};
   const int kr_i = p.KR / 16 - 1;
   const void* fn = kr_i == 0 ? reinterpret_cast<const void*>(head_bwd2_kernel<16>)
@@ -487,16 +579,16 @@ const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const
   if (cudaMemsetAsync(amax_ws, 0, 4, stream) != cudaSuccess) return "head_bwd: memset failed";
   absmax_kernel<<<num_sms * 4, 256, 0, stream>>>(dout, n_dout, amax_ws);
   const uint32_t tile_bytes = 2u * p.KR * 128;
-  const uint32_t fixed = 16384 + tile_bytes + kGroupsHB * (32768 + tile_bytes) + 4 * kGroupsHB * kRowScratchFloats * 4 +
-                         2048 + 1024;
+  const uint32_t fixed = 16384 + tile_bytes + kGroupsHB * (32768 + 2 * tile_bytes) + 2048 + 1024 +
+                         (p.KR > 32 ? 32 * 128 * kGroupsHB * 4 : 0);
   p.stages = kMaxStagesHB;
   while (p.stages > kGroupsHB && fixed + p.stages * tile_bytes > 227 * 1024) p.stages -= kGroupsHB;
   const uint32_t smem_bytes = fixed + p.stages * tile_bytes;
   const long long tiles = p.tiles_per_b * B;
   const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
-  if (kr_i == 0) head_bwd2_kernel<16><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, p);
-  else if (kr_i == 1) head_bwd2_kernel<32><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, p);
-  else head_bwd2_kernel<48><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, p);
+  if (kr_i == 0) head_bwd2_kernel<16><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
+  else if (kr_i == 1) head_bwd2_kernel<32><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
+  else head_bwd2_kernel<48><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }

@@ -1,5 +1,6 @@
 // Thin inline-PTX layer for sm_90a (Hopper): mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma.mma_async)
-// with shared-memory matrix descriptors, the row view of a wgmma accumulator used by the epilogues, system-scope
+// with shared-memory matrix descriptors or a register A operand, stmatrix, setmaxnreg, the row view of a wgmma
+// accumulator used by the epilogues, system-scope
 // release/acquire for the peer-memory (NVLink) kernels, and the GELU math shared by the kernels.
 //
 // Descriptor encodings follow the PTX ISA ("Matrix Descriptor Format" of wgmma): canonical SWIZZLE_128B layouts,
@@ -130,6 +131,13 @@ __device__ __forceinline__ uint64_t gdesc_mn128(uint32_t smem_addr, uint32_t lbo
 // wgmma: issue / ordering.  A warpgroup is four consecutive warps starting at a multiple of four; all 128 threads
 // execute every call below with identical operands.
 // ------------------------------------------------------------------------------------------
+// Per-warpgroup register budget (all 128 threads execute it): a TMA producer warpgroup gives registers back so
+// that the consumer warpgroups can hold fragments beyond the uniform per-thread limit of the launch.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N)); }
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
 template <int N>
@@ -281,6 +289,63 @@ __device__ __forceinline__ void wg_mma128(float (&acc)[R], int n, uint64_t da, u
                                           uint32_t scale_d) {
   wg_mma64<kF16, TA, TB, 0>(acc, n, da, db, scale_d);
   wg_mma64<kF16, TA, TB, R / 2>(acc, n, da + (a_half_bytes >> 4), db, scale_d);
+}
+
+// wgmma.mma_async m64nNk16, fp16 inputs, fp32 accumulators, A from REGISTERS (a[4]: the m64k16 A fragment of this
+// thread, see afrag_from_acc), B from shared memory.  N = 16 / 32 / 48.
+#define DFNO_WGMMA_RS(N, REGS, A, B, S, TB, ...)                                                                \
+  template <int kTB>                                                                                             \
+  __device__ __forceinline__ void wgmma_m64n##N##k16_f16_rs(float* d, const uint32_t (&a)[4], uint64_t db,       \
+                                                            uint32_t scale_d) {                                  \
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #S ", 0;\nwgmma.mma_async.sync.aligned.m64n" #N            \
+                 "k16.f32.f16.f16 {" REGS "}, {" A "}, %" #B ", p, 1, 1, %" #TB ";\n}\n"                         \
+                 : __VA_ARGS__                                                                                   \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(kTB));                 \
+  }
+DFNO_WGMMA_RS(16, "%0,%1,%2,%3,%4,%5,%6,%7", "%8,%9,%10,%11", 12, 13, 14,
+              "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]))
+DFNO_WGMMA_RS(32, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15", "%16,%17,%18,%19", 20, 21, 22,
+              "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]))
+DFNO_WGMMA_RS(48,
+              "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23",
+              "%24,%25,%26,%27", 28, 29, 30,
+              "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]))
+#undef DFNO_WGMMA_RS
+
+// acc[OFF .. OFF + N/2) (+)= A[64 x 16] (registers) . B[16 x N] (shared memory), N = 16, 32 or 48
+template <int N, int TB, int OFF, int R>
+__device__ __forceinline__ void wg_mma64_rs(float (&acc)[R], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  static_assert(OFF + N / 2 <= R, "accumulator too small");
+  if constexpr (N == 16) wgmma_m64n16k16_f16_rs<TB>(acc + OFF, a, db, scale_d);
+  else if constexpr (N == 32) wgmma_m64n32k16_f16_rs<TB>(acc + OFF, a, db, scale_d);
+  else { static_assert(N == 48, "N = 16, 32 or 48"); wgmma_m64n48k16_f16_rs<TB>(acc + OFF, a, db, scale_d); }
+}
+
+// The accumulator fragment of an m64nN wgmma is the A fragment of the next k16 step: register 4j + e holds row
+// l/4 + 8(e/2), column 8j + 2(l%4) + e%2 (per warp), and A register i of k16 step ks holds row l/4 + 8(i%2),
+// columns 16ks + 8(i/2) + 2(l%4) + {0, 1}.  So A register i of step ks is the packed pair acc[8ks + 2i, 8ks + 2i + 1]:
+// a[i] = f(acc[8ks + 2i], acc[8ks + 2i + 1], i), where f returns the f16x2 bits of the (transformed) pair.
+template <typename F>
+__device__ __forceinline__ void afrag_from_acc(const float* acc, int ks, uint32_t (&a)[4], F&& f) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) a[i] = f(acc[8 * ks + 2 * i], acc[8 * ks + 2 * i + 1], i);
+}
+
+// stmatrix: four 8 x 8 b16 matrices, matrix i from register r[i] of every lane (lane l holds row l/4, columns
+// 2(l%4), 2(l%4) + 1: the fragment layout above); lane 8i + k gives the shared address of row k of matrix i
+// (16 contiguous bytes).  The .trans form stores each matrix transposed: memory row k receives column k.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(r[0]),
+               "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(r[0]),
+               "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
 }
 
 // ------------------------------------------------------------------------------------------
