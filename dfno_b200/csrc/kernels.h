@@ -14,8 +14,9 @@ struct LiftDims {
 
 const char* lift_fwd(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
                      const float* b2, void* h, LiftDims d, int num_sms, cudaStream_t s);
+// dx (may be null): fp32 input gradient in x's layout, written (not accumulated)
 const char* lift_bwd(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
-                     const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2,
+                     const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2, float* dx,
                      LiftDims d, int num_sms, cudaStream_t s);
 // strided permutation of 32-bit words: dst walked in mixed-radix order (innermost digit first, strides in words)
 const char* permute_u32(const void* src, void* dst, int nd, const int* size, const long long* sstr,
@@ -39,7 +40,7 @@ const char* bypass_bwd_tc(const void* dout, const void* dout_cl, int cl_pitch, v
 
 // spectral channel mixing over the local mode slab: x,y bf16 [B, C, Q, 2]; w fp32 [C, C, Q, 2]
 const char* spectral_mix_fwd(const void* x, const float* w, void* y, int B, int C, long long Q, cudaStream_t s);
-// dx = dy * conj(w) ; dw (+)= conj(x) * dy summed over the batch
+// dx = dy * conj(w) ; dw (+)= conj(x) * dy summed over the batch (dw null: dx only, frozen weights)
 const char* spectral_mix_bwd(const void* x, const float* w, const void* dy, void* dx, float* dw, int accumulate,
                              int B, int C, long long Q, cudaStream_t s);
 

@@ -40,14 +40,18 @@ void lift_fwd(const at::Tensor& x, const at::Tensor& W1, const at::Tensor& b1, c
                        bptr(h), lift_dims(dims), sm_count(), cur_stream()), "lift_fwd");
 }
 
+// dx (optional): fp32 tensor of x's size, receives the input gradient
 void lift_bwd(const at::Tensor& x, const at::Tensor& W1, const at::Tensor& b1, const at::Tensor& W2,
               const at::Tensor& b2, const at::Tensor& dh, at::Tensor& gW1, at::Tensor& gb1, at::Tensor& gW2,
-              at::Tensor& gb2, const std::vector<int64_t>& dims) {
+              at::Tensor& gb2, const std::vector<int64_t>& dims, const c10::optional<at::Tensor>& dx) {
   TORCH_CHECK(x.is_cuda() && x.is_contiguous(), "x must be a contiguous CUDA tensor");
+  TORCH_CHECK(x.scalar_type() == at::kFloat || x.scalar_type() == at::kBFloat16, "x must be fp32 or bf16");
+  TORCH_CHECK(!dx || dx->numel() == x.numel(), "dx must have as many elements as x");
   c10::cuda::CUDAGuard guard(x.device());
   check(dfno::lift_bwd(x.data_ptr(), x.scalar_type() == at::kBFloat16, fptr(W1), fptr(b1), fptr(W2), fptr(b2),
-                       bptr(dh), fptr_mut(gW1), fptr_mut(gb1), fptr_mut(gW2), fptr_mut(gb2), lift_dims(dims),
-                       sm_count(), cur_stream()), "lift_bwd");
+                       bptr(dh), fptr_mut(gW1), fptr_mut(gb1), fptr_mut(gW2), fptr_mut(gb2),
+                       dx ? const_cast<float*>(fptr(*dx)) : nullptr, lift_dims(dims), sm_count(), cur_stream()),
+        "lift_bwd");
 }
 
 void bypass_gelu_fwd(const at::Tensor& h, at::Tensor& spec_pre, const at::Tensor& W,
@@ -95,11 +99,13 @@ void spectral_mix_fwd(const at::Tensor& x, const at::Tensor& w, at::Tensor& y, i
         "spectral_mix_fwd");
 }
 
-void spectral_mix_bwd(const at::Tensor& x, const at::Tensor& w, const at::Tensor& dy, at::Tensor& dx, at::Tensor& dw,
-                      bool accumulate, int64_t B, int64_t C, int64_t Q) {
+// dw None: dx only (frozen weights)
+void spectral_mix_bwd(const at::Tensor& x, const at::Tensor& w, const at::Tensor& dy, at::Tensor& dx,
+                      const c10::optional<at::Tensor>& dw, bool accumulate, int64_t B, int64_t C, int64_t Q) {
   c10::cuda::CUDAGuard guard(x.device());
-  check(dfno::spectral_mix_bwd(bptr(x), fptr(w), bptr(dy), bptr(dx), fptr_mut(dw), accumulate ? 1 : 0,
-                               static_cast<int>(B), static_cast<int>(C), Q, cur_stream()), "spectral_mix_bwd");
+  check(dfno::spectral_mix_bwd(bptr(x), fptr(w), bptr(dy), bptr(dx), dw ? const_cast<float*>(fptr(*dw)) : nullptr,
+                               accumulate ? 1 : 0, static_cast<int>(B), static_cast<int>(C), Q, cur_stream()),
+        "spectral_mix_bwd");
 }
 
 void adam_step(at::Tensor& p, const at::Tensor& g, at::Tensor& m, at::Tensor& v, double lr, double beta1, double beta2,
@@ -335,7 +341,8 @@ void register_ops(pybind11::module& m) {
   m.def("head_fwd", &head_fwd);
   m.def("head_bwd2", &head_bwd2);
   m.def("lift_fwd", &lift_fwd);
-  m.def("lift_bwd", &lift_bwd);
+  m.def("lift_bwd", &lift_bwd, py::arg("x"), py::arg("W1"), py::arg("b1"), py::arg("W2"), py::arg("b2"), py::arg("dh"),
+        py::arg("gW1"), py::arg("gb1"), py::arg("gW2"), py::arg("gb2"), py::arg("dims"), py::arg("dx") = c10::nullopt);
   m.def("bypass_gelu_fwd", &bypass_gelu_fwd);
   m.def("bypass_gelu_bwd", &bypass_gelu_bwd);
   m.def("bypass_fwd_tc", &bypass_fwd_tc);

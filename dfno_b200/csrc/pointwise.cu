@@ -7,7 +7,7 @@
 //
 //   lift_fwd        : x[B,Cin,X,Y,Z,Tin] -> h = gelu(W2 ._c gelu(W1 ._t x + b1) + b2)
 //                     (reference: linear1 -> gelu -> linear2 -> gelu, dfno.py:333-338; K15+K16)
-//   lift_bwd        : dh -> dW1, db1, dW2, db2 (recomputes the tiny activations)
+//   lift_bwd        : dh -> dW1, db1, dW2, db2 (recomputes the tiny activations), optionally dx
 //   bypass_gelu_fwd : pre = spec + W ._c h ; out = gelu(pre)         (K2 + K14, dfno.py:244,291)
 //   bypass_gelu_bwd : dpre = dout * gelu'(pre) ; dhb = W^T ._c dpre  (weight grad: kreduce GEMM)
 //   to_channels_last / from_channels_last : layout bridges for the projection head
@@ -141,12 +141,18 @@ lift_fwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
 // partials of the four quarters meet in two shuffles per value, and time-indexed sums are warp-reduced once per
 // t.  The loss gradient can be far below the fp16 range, so everything it multiplies is fp32; only the GELU'
 // evaluations are packed fp16.
-template <typename TIn, int C, int CIN, bool kRegs>
+//
+// kDx: also the input gradient dx[b, ci, x, y, z, ti] = sum_t W1[t, ti] e[ci, z, t] (fp32, same layout as x), with
+// e = dL/d(linear1 pre-activation).  After the quad shuffles every lane of the quad holds all 8 e[ci][z]; lane cg
+// owns z0 + 2cg and z0 + 2cg + 1, whose 2 * Tin values are contiguous in x's layout and written by this lane alone:
+// no atomics, no memset.  Tin == 1 keeps the 2 * CIN sums in registers over t; otherwise the first t stores and
+// later t add (read-modify-write of the lane's own run, which stays in L1 / L2).
+template <typename TIn, int C, int CIN, bool kRegs, bool kDx>
 __global__ void __launch_bounds__(128, (CIN == 1 ? 4 : 2))      // several input channels: more live values, no spills
 lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
                 const float* __restrict__ W2, const float* __restrict__ b2,
                 const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
-                float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d) {
+                float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx) {
   static_assert(C % 4 == 0, "the channels are split over four lanes");
   constexpr int CG = C / 4;
   __shared__ float sw[kLiftMaxW];
@@ -195,6 +201,12 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
     }
     const long long hc_stride = plane * d.T * d.Z;
     const __nv_bfloat16* gb = dh + ((static_cast<long long>(b) * C * plane + xy) * d.T) * d.Z + z0 + c0 * hc_stride;
+    float* dxl = kDx ? dx + (xb - x) + 2 * cg * d.Tin : nullptr;     // this lane's run [2 z][Tin] of ci = 0
+    float dxr[kDx && kRegs ? CIN : 1][2];
+    if (kDx && kRegs) {
+#pragma unroll
+      for (int ci = 0; ci < CIN; ++ci) dxr[ci][0] = dxr[ci][1] = 0.f;
+    }
     for (int t = 0; t < d.T; ++t) {
       __half2 a1[CIN][4];
       float a1f[CIN][8], g1f[CIN][8], da1[CIN][8];
@@ -265,6 +277,17 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
         float e[8];
 #pragma unroll
         for (int z = 0; z < 8; ++z) { e[z] = da1[ci][z] * g1f[ci][z]; sb1v += e[z]; }
+        float e0 = e[0], e1 = e[1];                           // e at this lane's two z (kDx)
+        if (kDx) {
+#pragma unroll
+          for (int k = 1; k < 4; ++k)
+            if (cg == k) { e0 = e[2 * k]; e1 = e[2 * k + 1]; }
+          if (kRegs) {
+            const float w = sW1[t];
+            dxr[ci][0] = fmaf(w, e0, dxr[ci][0]);
+            dxr[ci][1] = fmaf(w, e1, dxr[ci][1]);
+          }
+        }
         for (int ti = 0; ti < d.Tin; ++ti) {
           float xv[8];
           if (kRegs) {
@@ -278,10 +301,26 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
           for (int z = 0; z < 8; ++z) sres = fmaf(e[z], xv[z], sres);
           sres = warp_sum(own ? sres : 0.f);
           if (lane == 0) atomicAdd(&gsW1[t * d.Tin + ti], sres);
+          if (kDx && !kRegs && ok) {
+            float* p = dxl + ci * xci_stride + ti;
+            const float w = sW1[t * d.Tin + ti];
+            if (t == 0) {
+              p[0] = w * e0;
+              p[d.Tin] = w * e1;
+            } else {
+              p[0] = fmaf(w, e0, p[0]);
+              p[d.Tin] = fmaf(w, e1, p[d.Tin]);
+            }
+          }
         }
       }
       sb1v = warp_sum(own ? sb1v : 0.f);
       if (lane == 0) atomicAdd(&gsb1[t], sb1v);
+    }
+    if (kDx && kRegs && ok) {
+#pragma unroll
+      for (int ci = 0; ci < CIN; ++ci)
+        *reinterpret_cast<float2*>(dxl + ci * xci_stride) = make_float2(dxr[ci][0], dxr[ci][1]);
     }
   }
   __shared__ float gsW2[64 * 4 + 64];
@@ -611,13 +650,16 @@ const char* lift_fwd(const void* x, int x_is_bf16, const float* W1, const float*
 template <int C>
 static const char* lift_bwd_cin(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
                                 const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2,
-                                LiftDims d, int grid, bool regs, cudaStream_t s) {
-#define DFNO_LIFT_BWD2(T_, CIN_, R_)                                                                              \
-  lift_bwd_kernel<T_, C, CIN_, R_><<<grid, 128, 0, s>>>(static_cast<const T_*>(x), W1, b1, W2, b2,                \
-                                                        static_cast<const __nv_bfloat16*>(dh), gW1, gb1, gW2, gb2, d)
+                                float* dx, LiftDims d, int grid, bool regs, cudaStream_t s) {
+#define DFNO_LIFT_BWD3(T_, CIN_, R_, DX_)                                                                         \
+  lift_bwd_kernel<T_, C, CIN_, R_, DX_><<<grid, 128, 0, s>>>(static_cast<const T_*>(x), W1, b1, W2, b2,           \
+                                                             static_cast<const __nv_bfloat16*>(dh), gW1, gb1, gW2, \
+                                                             gb2, d, dx)
+#define DFNO_LIFT_BWD2(T_, CIN_, R_) \
+  if (dx) DFNO_LIFT_BWD3(T_, CIN_, R_, true); else DFNO_LIFT_BWD3(T_, CIN_, R_, false)
 #define DFNO_LIFT_BWD(CIN_)                                                                    \
-  if (x_is_bf16) { if (regs) DFNO_LIFT_BWD2(__nv_bfloat16, CIN_, true); else DFNO_LIFT_BWD2(__nv_bfloat16, CIN_, false); } \
-  else { if (regs) DFNO_LIFT_BWD2(float, CIN_, true); else DFNO_LIFT_BWD2(float, CIN_, false); }
+  if (x_is_bf16) { if (regs) { DFNO_LIFT_BWD2(__nv_bfloat16, CIN_, true); } else { DFNO_LIFT_BWD2(__nv_bfloat16, CIN_, false); } } \
+  else { if (regs) { DFNO_LIFT_BWD2(float, CIN_, true); } else { DFNO_LIFT_BWD2(float, CIN_, false); } }
   switch (d.Cin) {
     case 1: DFNO_LIFT_BWD(1); break;
     case 2: DFNO_LIFT_BWD(2); break;
@@ -627,18 +669,21 @@ static const char* lift_bwd_cin(const void* x, int x_is_bf16, const float* W1, c
   }
 #undef DFNO_LIFT_BWD
 #undef DFNO_LIFT_BWD2
+#undef DFNO_LIFT_BWD3
   return nullptr;
 }
 
 const char* lift_bwd(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
-                     const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2,
+                     const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2, float* dx,
                      LiftDims d, int num_sms, cudaStream_t s) {
   if (const char* e = lift_check(d)) return e;
+  if (dx && reinterpret_cast<uintptr_t>(dx) % 8) return "lift_bwd: dx must be 8-byte aligned";
   const long long nitems = static_cast<long long>(d.B) * d.X * d.Y * (d.Z / 8);
   const int grid = grid_for(4 * nitems, 128, num_sms, 4);          // four lanes per item (channel quarters)
   const bool regs = d.Tin == 1;
   const char* err = nullptr;
-  DFNO_DISPATCH_C(d.C, (err = lift_bwd_cin<kC>(x, x_is_bf16, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, d, grid, regs, s)));
+  DFNO_DISPATCH_C(d.C, (err = lift_bwd_cin<kC>(x, x_is_bf16, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, grid, regs,
+                                               s)));
   if (err) return err;
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);

@@ -6,7 +6,7 @@
 // batch sizes FNOs train at (B = 1..4) every mode owns a distinct C x C matrix that is used
 // once: the op is bound by streaming the fp32 weights (113-442 MB per block), i.e. a
 // bandwidth problem for plain FMA units with fully coalesced 8-byte loads, not a tensor-core
-// problem.  The backward makes ONE pass over R and produces both dX and dR.
+// problem.  The backward makes ONE pass over R and produces both dX and dR (dX alone for frozen weights).
 #include "sm90_ptx.cuh"
 #include "kernels.h"
 
@@ -51,7 +51,8 @@ mix_fwd_kernel(const uint32_t* __restrict__ x, const float2* __restrict__ w, uin
 }
 
 // one batch element per launch; dw (+)= conj(x) * dy ; dx = sum_o dy * conj(w)
-template <int C>
+// kDw = false (frozen weights): dx only -- no x read, no read-modify-write of dw.
+template <int C, bool kDw>
 __global__ void __launch_bounds__(kMixQ * kMixSplit)
 mix_bwd_kernel(const uint32_t* __restrict__ x, const float2* __restrict__ w, const uint32_t* __restrict__ dy,
                uint32_t* __restrict__ dx, float2* __restrict__ dw, int accumulate, long long Q) {
@@ -65,7 +66,7 @@ mix_bwd_kernel(const uint32_t* __restrict__ x, const float2* __restrict__ w, con
 #pragma unroll
     for (int ii = 0; ii < CG; ++ii) {
       const int i = i0 + ii;
-      const float2 xi = unpack_bf16x2(x[static_cast<long long>(i) * Q + q]);
+      const float2 xi = kDw ? unpack_bf16x2(x[static_cast<long long>(i) * Q + q]) : make_float2(0.f, 0.f);
       float2 r[C];
 #pragma unroll
       for (int o = 0; o < C; ++o) r[o] = __ldg(&w[(static_cast<long long>(i) * C + o) * Q + q]);
@@ -76,12 +77,14 @@ mix_bwd_kernel(const uint32_t* __restrict__ x, const float2* __restrict__ w, con
         // dy * conj(r)
         dr = fmaf(gv[o].x, r[o].x, dr); dr = fmaf(gv[o].y, r[o].y, dr);
         di = fmaf(gv[o].y, r[o].x, di); di = fmaf(-gv[o].x, r[o].y, di);
-        // conj(x) * dy
-        float2 g;
-        g.x = xi.x * gv[o].x + xi.y * gv[o].y;
-        g.y = xi.x * gv[o].y - xi.y * gv[o].x;
-        if (accumulate) { const float2 old = dw[widx]; g.x += old.x; g.y += old.y; }
-        dw[widx] = g;
+        if (kDw) {
+          // conj(x) * dy
+          float2 g;
+          g.x = xi.x * gv[o].x + xi.y * gv[o].y;
+          g.y = xi.x * gv[o].y - xi.y * gv[o].x;
+          if (accumulate) { const float2 old = dw[widx]; g.x += old.x; g.y += old.y; }
+          dw[widx] = g;
+        }
       }
       dx[static_cast<long long>(i) * Q + q] = pack_bf16x2(dr, di);
     }
@@ -123,8 +126,13 @@ const char* spectral_mix_bwd(const void* x, const float* w, const void* dy, void
     const uint32_t* gb = static_cast<const uint32_t*>(dy) + static_cast<long long>(b) * C * Q;
     uint32_t* dxb = static_cast<uint32_t*>(dx) + static_cast<long long>(b) * C * Q;
     const int acc = (accumulate || b > 0) ? 1 : 0;
-    DFNO_MIX_DISPATCH(C, (mix_bwd_kernel<kC><<<grid, block, 0, s>>>(xb, reinterpret_cast<const float2*>(w), gb, dxb,
-                                                                 reinterpret_cast<float2*>(dw), acc, Q)));
+    if (dw) {
+      DFNO_MIX_DISPATCH(C, (mix_bwd_kernel<kC, true><<<grid, block, 0, s>>>(xb, reinterpret_cast<const float2*>(w), gb,
+                                                                         dxb, reinterpret_cast<float2*>(dw), acc, Q)));
+    } else {
+      DFNO_MIX_DISPATCH(C, (mix_bwd_kernel<kC, false><<<grid, block, 0, s>>>(xb, reinterpret_cast<const float2*>(w), gb,
+                                                                          dxb, nullptr, 0, Q)));
+    }
   }
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);

@@ -259,7 +259,8 @@ class DistributedFNO(nn.Module):
 
     ``backend="auto"`` hands construction to the fused sm_90a engine when the device,
     dtype and partition are ones it covers (see :func:`dfno_b200.models.fused.supports`);
-    ``backend="torch"`` forces this portable implementation.
+    ``backend="torch"`` forces this portable implementation.  ``input_grad=True`` asks for dL/dx on either backend
+    (the fused engine refuses an input that requires grad without it).
     """
 
     def __new__(cls, *args, backend: str = "auto", **kwargs):
@@ -272,7 +273,9 @@ class DistributedFNO(nn.Module):
     def __init__(self, P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width: int,
                  modes: Sequence[int], num_blocks: int = 4, device=torch.device("cpu"),
                  dtype=torch.float32, plan: str = "reference", backend: str = "auto",
-                 init_seed: Optional[int] = None, fft_impl: str = "torch"):
+                 init_seed: Optional[int] = None, fft_impl: str = "torch", input_grad: bool = False):
+        # input_grad: accepted for constructor parity with the fused engine (which returns dL/dx only when asked);
+        # this backend always differentiates its input
         super().__init__()
         if init_seed is not None:       # reproducible draw (per rank; the fused engine's is partition independent)
             torch.manual_seed(int(init_seed) + 7919 * max(int(P_x.rank), 0))

@@ -507,13 +507,16 @@ class _FusedFn(torch.autograd.Function):
     """Autograd edge of the engine.  The saved activations live in ONE engine-owned buffer set, so a backward is
     only valid for the most recent saving forward: every such forward gets a generation number and a stale
     backward raises instead of silently using another forward's activations (micro-batch accumulation must run
-    forward -> backward per micro-batch, with ``accumulate_grads``)."""
+    forward -> backward per micro-batch, with ``accumulate_grads``).
+
+    With ``input_grad=True`` the backward also returns dL/dx, and a frozen ``theta`` (``requires_grad=False``)
+    gets a backward that computes dL/dx alone and leaves ``theta.grad`` untouched.  There is no double backward."""
 
     @staticmethod
     def forward(ctx, x, theta, eng, save):
-        if ctx.needs_input_grad[0]:
-            raise RuntimeError("the fused engine does not produce input gradients (dL/dx); use backend='torch' "
-                               "or detach the input")
+        if ctx.needs_input_grad[0] and not eng.input_grad:
+            raise RuntimeError("the fused engine does not produce input gradients (dL/dx) unless it is built with "
+                               "input_grad=True; use that, backend='torch', or detach the input")
         ctx.eng = eng
         if save:
             eng._generation += 1
@@ -526,24 +529,34 @@ class _FusedFn(torch.autograd.Function):
     def backward(ctx, dy):
         (x,) = ctx.saved_tensors
         eng = ctx.eng
+        if torch.is_grad_enabled():
+            raise RuntimeError("the fused engine has no double backward (create_graph=True); use backend='torch'")
         if ctx.generation != eng._generation:
             raise RuntimeError("backward through a fused-engine forward whose saved activations were overwritten by a "
                                "later forward (the engine keeps one set); run forward/backward pairs back to back")
+        want_dx, want_dtheta = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         # the engine writes straight into theta.grad's storage (no 2 GB autograd copy)
-        eng._backward(x, dy)
-        return None, None, None, None
+        dx = eng._backward(x, dy, input_grad=want_dx, theta_grad=want_dtheta)
+        if dx is not None:
+            dx = dx.view(x.shape).to(x.dtype)
+        return dx, None, None, None
 
 
 class FusedDistributedFNO(nn.Module):
     """Drop-in ``DistributedFNO`` on the fused sm_90a engine.  Same constructor; the forward
     takes this rank's ``[B, C_in, X, Y_local, Z, T_in]`` shard (fp32 or bf16, CUDA) and returns
-    ``[B, 1, X, Y_local, Z, T_out]`` in fp32."""
+    ``[B, 1, X, Y_local, Z, T_out]`` in fp32.
+
+    ``input_grad=True``: an input that requires grad gets dL/dx (in its own dtype and shape) from the backward, for
+    surrogate inversion and sensitivity studies.  With ``theta.requires_grad_(False)`` that backward computes dL/dx
+    only and leaves ``theta.grad`` as it was.  Without it (the default) such an input is refused."""
 
     def __init__(self, P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width: int,
                  modes: Sequence[int], num_blocks: int = 4, device=torch.device("cuda"),
                  dtype=torch.bfloat16, plan: Optional[str] = None, backend: str = "fused",
-                 use_p2p: Optional[bool] = None, init_seed: Optional[int] = None):
+                 use_p2p: Optional[bool] = None, init_seed: Optional[int] = None, input_grad: bool = False):
         super().__init__()
+        self.input_grad = bool(input_grad)
         ok, why = supports(P_x, in_shape, out_timesteps, width, modes)
         if not ok:
             raise ValueError(f"fused engine cannot run this configuration: {why}")
@@ -731,7 +744,9 @@ class FusedDistributedFNO(nn.Module):
             self._saved["hcl"] = torch.zeros(pl.npos, pl.CP, **bf)                # last block out, channels-last
             self.ws["dhb"] = torch.empty(pl.n_act, **bf)
             self.ws["gcl"] = torch.empty(pl.npos, pl.CP, **bf)
-        self.grad_flat = torch.zeros(pl.n_theta, device=self.device, dtype=torch.float32)
+        # theta.grad's storage: allocated by the first backward that produces weight gradients (a frozen network
+        # used for inversion never needs it)
+        self.grad_flat = None
         self.accumulate_grads = False          # True: keep adding into theta.grad across backward calls
         self._train_bufs_ready = True
 
@@ -776,12 +791,14 @@ class FusedDistributedFNO(nn.Module):
         if st.get("barrier_after"):
             self.barrier()
 
-    def _spectral_chain(self, src, dst, block: int, adj: bool, add=None, fuse: Optional[dict] = None) -> None:
+    def _spectral_chain(self, src, dst, block: int, adj: bool, add=None, fuse: Optional[dict] = None,
+                        grad: Optional[torch.Tensor] = None) -> None:
         """src (engine layout) -> truncated spectrum -> channel mix -> dst (engine layout).
 
         ``fuse`` (round-2 dataflow): the last stage becomes ``spectral_out`` -- inverse z-DFT + bypass conv of
         ``fuse["h"]`` with ``fuse["W"]`` (transposed in the adjoint chain) (+ GELU, pre-activation kept in
-        ``fuse["pre"]``) -- instead of a plain row-major GEMM."""
+        ``fuse["pre"]``) -- instead of a plain row-major GEMM.  ``grad`` (adjoint chain): the flat gradient buffer
+        whose spectral segment the mix backward writes; ``None`` runs the dx-only mix backward (frozen weights)."""
         pl = self.plan
         ws = self.ws
         s3 = self._saved["S3"][block] if (self._train_bufs_ready and not self._eval_mode) else ws["S3w"]
@@ -799,7 +816,7 @@ class FusedDistributedFNO(nn.Module):
                 self._C.permute_u32(bufs[st["src"]], bufs[st["dst"]], st["size"], st["sstr"], st["dstr"])
             elif st["name"] == "mix":
                 if adj:
-                    gR = self._seg(f"blocks.{block}.spectral", self.grad_flat)
+                    gR = None if grad is None else self._seg(f"blocks.{block}.spectral", grad)
                     self._C.spectral_mix_bwd(s3, R, bufs["S3"], bufs["S4"], gR, getattr(self, "_acc", False), pl.B, pl.C, pl.Q)
                 else:
                     self._C.spectral_mix_fwd(bufs["S3"], R, bufs["S4"], pl.B, pl.C, pl.Q)
@@ -861,11 +878,10 @@ class FusedDistributedFNO(nn.Module):
                          self._seg("linear3.b"), self._w4b4(), 0.0)
         return out
 
-    def _head_backward(self, hcl: torch.Tensor, dy: torch.Tensor, gcl: torch.Tensor) -> None:
+    def _head_backward(self, hcl: torch.Tensor, dy: torch.Tensor, gcl: torch.Tensor, g: torch.Tensor) -> None:
         pl = self.plan
         w3, w3t = self._head_operators()
         R, SR = self._head_row_digits()
-        g = self.grad_flat
         self._C.head_bwd(hcl, pl.npos, pl.C, pl.CP, w3, w3t, self._seg("linear3.b"),
                          self._seg("linear4.W").view(-1), dy, R, SR, gcl,
                          self._seg("linear3.W", g), self._seg("linear3.b", g),
@@ -930,7 +946,12 @@ class FusedDistributedFNO(nn.Module):
             out = self._head_forward(hcl)
             return out.squeeze(2) if self.five_d else out
 
-    def _backward(self, x: torch.Tensor, dy: torch.Tensor) -> torch.Tensor:
+    def _backward(self, x: torch.Tensor, dy: torch.Tensor, input_grad: bool = False,
+                  theta_grad: bool = True) -> Optional[torch.Tensor]:
+        """Backward of the last saving forward.  ``theta_grad``: the weight gradients go to ``grad_flat``, which
+        becomes ``theta.grad``.  Otherwise (frozen weights) ``theta.grad`` is left as it was: the spectral-weight
+        gradients are not formed and the small segment's kernels accumulate into a scratch buffer.  ``input_grad``:
+        returns dL/dx as fp32 in the engine's local 6-D input shape (else ``None``)."""
         pl, C_ = self.plan, self._C
         x = x.contiguous()
         if x.dtype not in (torch.float32, torch.bfloat16):
@@ -940,12 +961,20 @@ class FusedDistributedFNO(nn.Module):
         self._eval_mode = False
         hs, pres = self._saved["h"], self._saved["pre"]
         g = self.ws["g"]
-        if not (self.accumulate_grads and self.theta.grad is self.grad_flat):
-            # spectral gradients are overwritten by the mix backward; only the small,
-            # atomically accumulated segment needs clearing
-            self.grad_flat[:pl.n_small].zero_()
-        self._acc = bool(self.accumulate_grads and self.theta.grad is self.grad_flat)
-        gf = self.grad_flat
+        if theta_grad:
+            if self.grad_flat is None:
+                self.grad_flat = torch.zeros(pl.n_theta, device=self.device, dtype=torch.float32)
+            if not (self.accumulate_grads and self.theta.grad is self.grad_flat):
+                # spectral gradients are overwritten by the mix backward; only the small,
+                # atomically accumulated segment needs clearing
+                self.grad_flat[:pl.n_small].zero_()
+            self._acc = bool(self.accumulate_grads and self.theta.grad is self.grad_flat)
+            gf = gR = self.grad_flat
+        else:
+            if "g_small" not in self.ws:
+                self.ws["g_small"] = torch.empty(pl.n_small, device=self.device, dtype=torch.float32)
+            gf, gR = self.ws["g_small"], None
+            gf.zero_()
         if self.fused_pw:
             nb = self.num_blocks
             with _nvtx("dfno.head.bwd"):
@@ -961,15 +990,15 @@ class FusedDistributedFNO(nn.Module):
                     C_.dpre_dw(g, pres[k], hs[k], self._seg(f"blocks.{k}.linear.W", gf), pl.B, pl.C, L, pl.Z)
                     # adjoint chain; its last GEMM adds W^T dpre (the bypass input gradient) in the same accumulator
                     self._spectral_chain(pres[k], g, k, adj=True,
-                                         fuse=dict(h=pres[k], W=self._seg(f"blocks.{k}.linear.W")))
+                                         fuse=dict(h=pres[k], W=self._seg(f"blocks.{k}.linear.W")), grad=gR)
         else:
             hcl, dhb, gcl = self._saved["hcl"], self.ws["dhb"], self.ws["gcl"]
             with _nvtx("dfno.head.bwd"):
-                self._head_backward(hcl, dy.contiguous().float(), gcl)
+                self._head_backward(hcl, dy.contiguous().float(), gcl, gf)
             for k in reversed(range(self.num_blocks)):
                 last = k == self.num_blocks - 1
                 Wb = self._seg(f"blocks.{k}.linear.W")
-                gW = self._seg(f"blocks.{k}.linear.W", self.grad_flat)
+                gW = self._seg(f"blocks.{k}.linear.W", gf)
                 if self.use_tc_bypass:
                     # one wgmma kernel: dpre (over pre), dhb = W^T dpre, dW accumulated in registers
                     C_.bypass_bwd_tc(None if last else g, gcl if last else None, pl.CP, pres[k], hs[k],
@@ -978,26 +1007,29 @@ class FusedDistributedFNO(nn.Module):
                     # dpre overwrites pre (same thread reads then writes each element)
                     C_.bypass_gelu_bwd(None if last else g, gcl if last else None, pl.CP, pres[k], Wb, pres[k], dhb,
                                        pl.B, pl.C, pl.S)
-                    for b in range(pl.B):
-                        sl = slice(b * pl.C * pl.S, (b + 1) * pl.C * pl.S)
-                        C_.kreduce_gemm(pres[k][sl], pl.S, pl.C, hs[k][sl], pl.S, pl.C, pl.S, gW)
+                    if theta_grad:          # this GEMM only forms the bypass weight gradient
+                        for b in range(pl.B):
+                            sl = slice(b * pl.C * pl.S, (b + 1) * pl.C * pl.S)
+                            C_.kreduce_gemm(pres[k][sl], pl.S, pl.C, hs[k][sl], pl.S, pl.C, pl.S, gW)
                 with _nvtx(f"dfno.block{k}.spectral.bwd"):
-                    self._spectral_chain(pres[k], g, k, adj=True, add=dhb)
+                    self._spectral_chain(pres[k], g, k, adj=True, add=dhb, grad=gR)
+        # lift: fp32 dx in x's (local, 6-D) layout, written whole by the kernel -- no memset
+        dx = torch.empty(x.shape, device=self.device, dtype=torch.float32) if input_grad else None
         C_.lift_bwd(x, self._seg("linear1.W"), self._seg("linear1.b"), self._seg("linear2.W"),
-                    self._seg("linear2.b"), g, self._seg("linear1.W", self.grad_flat),
-                    self._seg("linear1.b", self.grad_flat), self._seg("linear2.W", self.grad_flat),
-                    self._seg("linear2.b", self.grad_flat), self._lift_dims())
-        self._sync_small_grads()
-        self.theta.grad = self.grad_flat
-        return self.grad_flat
+                    self._seg("linear2.b"), g, self._seg("linear1.W", gf), self._seg("linear1.b", gf),
+                    self._seg("linear2.W", gf), self._seg("linear2.b", gf), self._lift_dims(), dx)
+        # the same reduction on every rank either way, so ranks that disagree about theta.requires_grad still pair
+        # up their peer barriers
+        self._sync_small_grads(gf[:pl.n_small])
+        if theta_grad:
+            self.theta.grad = self.grad_flat
+        return dx
 
-    def _sync_small_grads(self) -> None:
+    def _sync_small_grads(self, small: torch.Tensor) -> None:
         """Sum the replicated pointwise-weight gradients over the pencil (the SumReduce side
         of the reference's BroadcastedLinear, once per step instead of per layer)."""
         if self.world <= 1:
             return
-        pl = self.plan
-        small = self.grad_flat[:pl.n_small]
         if self.use_p2p:
             self.allreduce_small_(small)
         else:
@@ -1021,7 +1053,7 @@ class FusedDistributedFNO(nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if self.R_in is not None:
             x = self.R_in(x.contiguous())
-        save = bool(torch.is_grad_enabled() and self.theta.requires_grad)
+        save = bool(torch.is_grad_enabled() and (self.theta.requires_grad or (self.input_grad and x.requires_grad)))
         y = _FusedFn.apply(x, self.theta, self, save)
         if self.R_out is not None:
             y = self.R_out(y)
