@@ -68,7 +68,7 @@ def measure(staged):
         net.sym_S1.peer_ptrs, net.sym_T1.peer_ptrs = peer_saved
     net.barrier = barrier_saved
     bytes_out = (pl.n_S1 + pl.n_T1 * pl.mt // pl.mtp) * 2 * (N - 1) // N      # bf16 bytes leaving this rank per chain
-    res = {"n_gpus": N, "staged_scatter": bool(net.staged_scatter), "spectral_chain_ms": t_comm, "spectral_chain_comm_off_ms": t_local,
+    res = {"n_gpus": N, "staged_scatter": net.plan.staged, "spectral_chain_ms": t_comm, "spectral_chain_comm_off_ms": t_local,
            "exposed_all_to_all_ms_per_spectral_conv": max(t_comm - t_local, 0.0),
            "bytes_leaving_rank_per_chain": bytes_out,
            "link_time_at_450GBps_datasheet_ms": bytes_out / 450e9 * 1e3,

@@ -3,7 +3,7 @@
 # benchmarks/launch-summit.sh).  Environment knobs:
 #   DFNO_BENCH_BACKEND=auto|fused|torch   engine selection (default auto: fused when supported)
 #   DFNO_P2P_REPARTITION=0                portable backend: NCCL all_to_all instead of peer-memory push
-#   DFNO_STAGED_SCATTER=0|1|r2|r3         fused engine: direct / staged peer layout, or only one transpose staged (default auto)
+#   DFNO_STAGED_SCATTER=0|1               fused engine: direct / staged peer layout (default: staged from 8 ranks)
 #   DFNO_NVTX=1                           NVTX ranges around the engine phases (lift / block k spectral, bypass / head)
 #   DFNO_SYNC_TIMERS=1                    dt_comm timers synchronise the device around collectives
 #   PROFILE=<dir>                         wrap 1-GPU points in `ncu --set full` (see bench.sh)

@@ -212,6 +212,14 @@ class EnginePlan:
         self.npos = B * self.S
         self.Q = self.kzl * self.mt * self.KY * self.KX    # local modes
         self.CP = (C + 7) // 8 * 8                         # channels-last pitch (16-byte rows)
+        # Routes, decided by the shape: the module runs them, memory_bytes / cost_model size them.  fused_pw: the round-2
+        # pointwise dataflow (the chain's last GEMM also applies bypass conv + GELU, csrc/spectral_out_sm90.cu), whose
+        # inverse z-DFT takes K = 2*KZ <= 128; else round 1's separate bypass and channels-last head.  tc_bypass (round
+        # 1 only): whole 128-position tiles for the tensor-core bypass, else CUDA cores + kreduce_gemm.  staged: chain()'s
+        # staged peer layout pays once the direct NVLink runs get short (many ranks) and costs a permutation with few.
+        self.fused_pw = 2 * self.KZ <= 128
+        self.tc_bypass = self.S % 128 == 0
+        self.staged = world >= 8
         # element counts (bf16 unless noted)
         BC, Yl, kzl, mt, mtp = self.BC, self.Yl, self.kzl, self.mt, self.mtp
         self.n_act = BC * self.S
@@ -260,8 +268,7 @@ class EnginePlan:
         """The GEMM stages of one spectral convolution (forward *or* adjoint: only the operator
         matrices and the end buffers differ).  Strides in bf16 elements.
 
-        ``staged`` (multi-GPU; ``True``, or ``"r2"`` / ``"r3"`` for one transpose only) changes how the pencil
-        transposes cross NVLink: instead of
+        ``staged`` (multi-GPU) changes how both pencil transposes cross NVLink: instead of
         interleaving directly into the consumer layout (64- / 40-byte runs per destination row)
         every source rank deposits its contribution as long contiguous runs into a per-source
         block of a staging buffer (``S1s`` / ``T1s``, >= 512-byte runs), and a tiny local
@@ -271,11 +278,8 @@ class EnginePlan:
         P, r = self.world, self.rank
         m_loc = kzl * mt
         Tp = self.Tp
-        # ``staged``: False / True (both transposes) / "r2" / "r3" (only that transpose through a staging block)
-        staged_r2 = staged is True or staged == "r2"
-        staged_r3 = staged is True or staged == "r3"
         st = []
-        if not staged_r2:
+        if not staged:
             st.append(dict(name="G1a", src="src", dst="Z1", M=BC * X * Yl * T, K=Z, lda=Z, N=2 * KZ, op="G1a",
                            scatter=ScatterSpec(rows=[(T, 2), (Yl, 2 * Tp), (BC * X, KZ * Yl * Tp * 2)],
                                                cols=(KZ, Yl * Tp * 2, 0))))
@@ -308,7 +312,7 @@ class EnginePlan:
             st.append(dict(name="iG3", src="S4", dst="T2", M=BC * m_loc * KY, K=2 * KX, lda=2 * KX, N=2 * X, op="iG3",
                            scatter=ScatterSpec(rows=[(KY, 2), (m_loc, KY * 2), (BC, X * m_loc * KY * 2)],
                                                cols=(X, m_loc * KY * 2, 0))))
-        if not staged_r3:
+        if not staged:
             st.append(dict(name="iG2", src="T2" if self.has_x else "S4", dst="T1", M=BC * X * m_loc, K=2 * KY,
                            lda=2 * KY, N=2 * Y, op="iG2",
                            scatter=ScatterSpec(rows=[(mt, 2), (kzl, mtp * 2), (X, Yl * KZ * mtp * 2),
@@ -355,25 +359,24 @@ class EnginePlan:
                 continue
         raise ValueError(f"stage {st['name']}: no column split of {npairs} pairs fits {self.max_n}")
 
-    def memory_bytes(self, train: bool = True, staged: Optional[bool] = None, legacy: bool = False) -> Dict[str, int]:
-        """Per-rank device memory of the engine for this plan, by category (bytes).  Mirrors the
+    def memory_bytes(self, train: bool = True) -> Dict[str, int]:
+        """Per-rank device memory of the engine for this plan and its routes, by category (bytes).  Mirrors the
         allocations of :class:`FusedDistributedFNO` (``__init__``, ``_ensure_train_buffers``,
         ``_ensure_eval_buffers``) and :class:`FusedAdam`; used to size shards for the 80 GB of an H100
         before anything is allocated."""
         if self.num_blocks is None:
             raise RuntimeError("call finish(num_blocks) first")
-        if staged is None:
-            staged = self.world >= 8
         nb, bf, f32 = self.num_blocks, 2, 4
+        legacy = not self.fused_pw
         cl = self.npos * self.CP                                   # channels-last slab
         out = {
             "parameters": self.n_theta * f32,
             "workspaces": (max(self.n_Z1, self.n_U) + self.n_S1 + self.n_T1 + self.n_S2 + 2 * self.n_S3 + self.n_T2) * bf,
-            "staging": ((self.n_S1 * bf if staged in (True, "r2") else 0) + (self.n_T1 * bf if staged in (True, "r3") else 0)
-                        if self.world > 1 else 0) + (self.n_small * f32 if self.world > 1 else 0),
+            "staging": (((self.n_S1 + self.n_T1) * bf if self.staged else 0) + self.n_small * f32
+                        if self.world > 1 else 0),
             "input_output": self.B * self.S // self.T * self.Cin * self.Tin * f32 + self.B * self.S * f32,
         }
-        if train and legacy:            # round-1 dataflow (DFNO_POINTWISE=legacy): channels-last head, separate bypass
+        if train and legacy:            # round-1 dataflow: channels-last head, separate bypass
             out["saved_activations"] = (2 * nb * self.n_act + nb * self.n_S3 + cl) * bf
             out["backward_workspaces"] = (2 * self.n_act + cl) * bf
         elif train:                     # block inputs + last output, pre-activations, spectra entering the mix
@@ -388,9 +391,9 @@ class EnginePlan:
         return out
 
     def cost_model(self, hbm_gbs: float = H100_COPY_GBS, nvlink_gbs: Optional[float] = None,
-                   staged: Optional[bool] = None, legacy: bool = False, front: bool = False) -> Dict[str, object]:
-        """Bytes every kernel of one training step must move (per rank) and the resulting floors.
-        ``front``: G1a + G1b run as the single ``spectral_in`` kernel (Z1 stays on the SM).
+                   front: bool = False) -> Dict[str, object]:
+        """Bytes every kernel of one training step must move (per rank) on this plan's routes and the resulting
+        floors.  ``front``: G1a + G1b run as the single ``spectral_in`` kernel (Z1 stays on the SM).
 
         Pure bookkeeping of the dataflow in :class:`FusedDistributedFNO` -- each stage reads its input
         buffer and writes its output buffer once; nothing is assumed to stay in L2 (the working set of a
@@ -401,9 +404,8 @@ class EnginePlan:
         issued from GEMM epilogues), so the step floor is ``max`` of the two per chain, not their sum."""
         if self.num_blocks is None:
             raise RuntimeError("call finish(num_blocks) first")
-        if staged is None:
-            staged = self.world >= 8
         nb, bf, f32 = self.num_blocks, 2, 4
+        legacy = not self.fused_pw
         P = self.world
         act, cl = self.n_act * bf, self.npos * self.CP * bf
         Z1, S1, S2, S3, T2, U = (self.n_Z1 * bf, self.n_S1 * bf, self.n_S2 * bf, self.n_S3 * bf, self.n_T2 * bf,
@@ -419,10 +421,8 @@ class EnginePlan:
             chain = [c for c in chain if c[0] not in ("G3", "iG3")]
         if legacy:
             chain.append(("iG1a", U + act, 0))
-        if P > 1 and staged in (True, "r2"):
-            chain.append(("permS1", 2 * S1, 0))
-        if P > 1 and staged in (True, "r3"):
-            chain.append(("permT1", 2 * T1, 0))
+        if P > 1 and self.staged:
+            chain += [("permS1", 2 * S1, 0), ("permT1", 2 * T1, 0)]
         st = [(n, 2 * nb, b, l) for n, b, l in chain]                  # forward + adjoint chain per block
         st += [("spectral_mix fwd", nb, 2 * S3 + W, 0), ("spectral_mix bwd", nb, 3 * S3 + 2 * W, 0),
                ("lift fwd", 1, act, 0), ("lift bwd", 1, act, 0), ("adam", 1, 7 * self.n_theta * f32, 0)]
@@ -624,38 +624,42 @@ class FusedDistributedFNO(nn.Module):
         self._saved: Dict[str, torch.Tensor] = {}
         self._train_bufs_ready = False
         self._generation = 0                     # number of saving forwards so far (see _FusedFn)
-        # staged peer layout (long NVLink runs + a local permutation): it pays when the direct runs get short,
-        # i.e. with many ranks, and costs a permutation pass with few; "auto" = on from 8 ranks.
-        _st = os.environ.get("DFNO_STAGED_SCATTER", "auto").lower()
-        mode = (self.world >= 8) if _st == "auto" else (_st if _st in ("r2", "r3") else _st != "0")
-        self.staged_scatter = mode if self.world > 1 else False      # False / True / "r2" / "r3"
-        self.chain_desc = pl.chain(staged=self.staged_scatter)
+        # DFNO_STAGED_SCATTER=0|1 overrides the plan's peer layout (A/B runs, the 8-rank layout on fewer GPUs); it is
+        # written into the plan so that its memory and cost figures describe the layout that runs
+        st = os.environ.get("DFNO_STAGED_SCATTER")
+        if st is not None:
+            if st not in ("0", "1"):
+                raise ValueError(f"DFNO_STAGED_SCATTER must be 0 or 1, got {st!r}")
+            pl.staged = st == "1" and self.world > 1
+        self.chain_desc = pl.chain(staged=pl.staged)
         # peers write the staging blocks; the consumer-side S1 / T1 become local buffers
-        if self.staged_scatter is True or self.staged_scatter == "r2":
+        if pl.staged:
             self.ws["S1s"] = self.ws["S1"]
             self.ws["S1"] = torch.empty(pl.n_S1, **bf)
-        if self.staged_scatter is True or self.staged_scatter == "r3":
             self.ws["T1s"] = self.ws["T1"]
             self.ws["T1"] = torch.zeros(pl.n_T1, **bf)
-        self.use_tc_bypass = (pl.S % 128 == 0 and pl.C <= 32 and os.environ.get("DFNO_TC_BYPASS", "1") != "0")
-        # round-2 dataflow: the last GEMM of every chain also applies the bypass conv (+ GELU), and the head reads
-        # the channel-major activation directly (csrc/spectral_out_sm90.cu, dpre_dw_sm90.cu, head_sm90.cu).
-        # DFNO_POINTWISE=legacy keeps round 1's separate bypass / channels-last head kernels for A/B runs.
-        self.fused_pw = os.environ.get("DFNO_POINTWISE", "fused").lower() != "legacy" and 2 * pl.KZ <= 128
         # the first two GEMMs of every chain (z-DFT, t-DFT) + the transpose R2 as ONE kernel that keeps Z1 on the SM
-        # (csrc/spectral_in_sm90.cu); DFNO_FRONT=legacy keeps the two dft_gemm launches for A/B runs.
-        self.front = None
-        if os.environ.get("DFNO_FRONT", "fused").lower() != "legacy":
-            self.front = self._front_plan()
+        # (csrc/spectral_in_sm90.cu); None where spectral_in_check refuses the shape (e.g. T > 64), and then G1a + G1b
+        # run as two dft_gemm launches
+        self.front = self._front_plan()
+
+    @property
+    def fused_pw(self) -> bool:
+        """The round-2 pointwise dataflow runs (else the round-1 kernels); decided by the plan from the shape."""
+        return self.plan.fused_pw
+
+    @property
+    def use_tc_bypass(self) -> bool:
+        """The round-1 route runs its bypass on the tensor core; decided by the plan from the shape."""
+        return self.plan.tc_bypass
 
     def _front_plan(self) -> Optional[dict]:
         """Destination view of ``spectral_in`` for this plan's S1 layout (direct or staged), or None when the kernel
         does not support the shape (then G1a + G1b run as separate GEMMs)."""
         pl = self.plan
         P, r = max(self.world, 1), self.rank
-        staged_r2 = self.staged_scatter is True or self.staged_scatter == "r2"
         X, Y, Yl, mt, kzl = pl.X, pl.Y, pl.Yl, pl.mt, pl.kzl
-        if staged_r2:        # S1s[bc, kz', kt, r_src, x, y_loc, ri] on the rank owning kz
+        if pl.staged:        # S1s[bc, kz', kt, r_src, x, y_loc, ri] on the rank owning kz
             dstr = [Yl * 2, P * X * Yl * 2, mt * P * X * Yl * 2, kzl * mt * P * X * Yl * 2]
             off = r * X * Yl * 2
         else:                # S1[bc, kz', kt, x, y, ri]
@@ -668,7 +672,7 @@ class FusedDistributedFNO(nn.Module):
                                         pl.BC, X, Yl, pl.T, pl.Z, pl.KZ, mt)
         if why:
             return None
-        return dict(dstr=dstr, off=off, dst="S1s" if staged_r2 else "S1")
+        return dict(dstr=dstr, off=off, dst="S1s" if pl.staged else "S1")
 
     def _front(self, src: torch.Tensor, adj: bool) -> None:
         pl, fr = self.plan, self.front
@@ -734,11 +738,11 @@ class FusedDistributedFNO(nn.Module):
         bf = dict(device=self.device, dtype=torch.bfloat16)
         nb = self.num_blocks
         # block inputs (+ the last block's output, which the head reads, in the fused pointwise dataflow)
-        self._saved["h"] = [torch.empty(pl.n_act, **bf) for _ in range(nb + (1 if self.fused_pw else 0))]
+        self._saved["h"] = [torch.empty(pl.n_act, **bf) for _ in range(nb + (1 if pl.fused_pw else 0))]
         self._saved["pre"] = [torch.empty(pl.n_act, **bf) for _ in range(nb)]     # pre-activations
         self._saved["S3"] = [torch.empty(pl.n_S3, **bf) for _ in range(nb)]       # spectra entering the mix
         self.ws["g"] = torch.empty(pl.n_act, **bf)
-        if self.fused_pw:
+        if pl.fused_pw:
             self.ws["amax"] = torch.zeros(1, device=self.device, dtype=torch.int32)
         else:
             self._saved["hcl"] = torch.zeros(pl.npos, pl.CP, **bf)                # last block out, channels-last
@@ -756,7 +760,7 @@ class FusedDistributedFNO(nn.Module):
         pl = self.plan
         bf = dict(device=self.device, dtype=torch.bfloat16)
         self.ws["eval_h"] = [torch.empty(pl.n_act, **bf) for _ in range(2)]
-        if not self.fused_pw:
+        if not pl.fused_pw:
             self.ws["eval_pre"] = torch.empty(pl.n_act, **bf)
             if "hcl" not in self._saved:
                 self._saved["hcl"] = torch.zeros(pl.npos, pl.CP, **bf)
@@ -917,7 +921,7 @@ class FusedDistributedFNO(nn.Module):
         with _nvtx("dfno.lift"):
             C_.lift_fwd(x, self._seg("linear1.W"), self._seg("linear1.b"), self._seg("linear2.W"),
                         self._seg("linear2.b"), hs[0], self._lift_dims())
-        if self.fused_pw:
+        if pl.fused_pw:
             for k in range(nb):
                 with _nvtx(f"dfno.block{k}"):
                     self._spectral_chain(hs[k], hs[k + 1], k, adj=False,
@@ -936,7 +940,7 @@ class FusedDistributedFNO(nn.Module):
                 self._spectral_chain(hs[k], pres[k], k, adj=False)
             Wb = self._seg(f"blocks.{k}.linear.W")
             with _nvtx(f"dfno.block{k}.bypass_gelu"):
-                if self.use_tc_bypass:
+                if pl.tc_bypass:
                     C_.bypass_fwd_tc(hs[k], pres[k], self._wpad(Wb), None if last else hs[k + 1],
                                      hcl if last else None, pl.CP, pl.B, pl.C, pl.S, save)
                 else:
@@ -975,7 +979,7 @@ class FusedDistributedFNO(nn.Module):
                 self.ws["g_small"] = torch.empty(pl.n_small, device=self.device, dtype=torch.float32)
             gf, gR = self.ws["g_small"], None
             gf.zero_()
-        if self.fused_pw:
+        if pl.fused_pw:
             nb = self.num_blocks
             with _nvtx("dfno.head.bwd"):
                 w3a, w3t = self._head_operators_cm()
@@ -999,7 +1003,7 @@ class FusedDistributedFNO(nn.Module):
                 last = k == self.num_blocks - 1
                 Wb = self._seg(f"blocks.{k}.linear.W")
                 gW = self._seg(f"blocks.{k}.linear.W", gf)
-                if self.use_tc_bypass:
+                if pl.tc_bypass:
                     # one wgmma kernel: dpre (over pre), dhb = W^T dpre, dW accumulated in registers
                     C_.bypass_bwd_tc(None if last else g, gcl if last else None, pl.CP, pres[k], hs[k],
                                      self._wpad(Wb.t()), dhb, gW, pl.B, pl.C, pl.S)

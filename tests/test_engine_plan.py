@@ -89,8 +89,7 @@ def _run_chain(plans, ops, src, weights, adj=False, staged=False):
 
 @pytest.mark.parametrize("P,staged,max_n", [(1, False, 256), (2, False, 256), (4, False, 256), (2, True, 256),
                                              (4, True, 256), (1, False, 8), (2, False, 8), (4, False, 8),
-                                             (4, True, 8), (2, True, 8), (1, False, 6), (2, True, 6), (4, False, 6),
-                                             (4, "r3", 256), (2, "r2", 256), (4, "r2", 8)])
+                                             (4, True, 8), (2, True, 8), (1, False, 6), (2, True, 6), (4, False, 6)])
 def test_stage_plan_reproduces_spectral_convolution(P, staged, max_n):
     """``max_n`` below the real limit forces the column-part path (used on the GPU for axes > 128)."""
     import dfno_b200 as d
@@ -142,7 +141,7 @@ def test_stage_plan_reproduces_spectral_convolution(P, staged, max_n):
     assert abs(lhs - rhs) < 1e-9 * max(1.0, abs(lhs)), (lhs, rhs)
 
 
-@pytest.mark.parametrize("P,staged", [(1, False), (2, False), (4, True), (2, "r3")])
+@pytest.mark.parametrize("P,staged", [(1, False), (2, False), (4, True), (2, True)])
 def test_stage_plan_2d_plus_time_runs_as_singleton_x(P, staged):
     """A 5-D problem [B, C, X', Y', T] is the 6-D engine plan with X = 1: the x stages vanish and G2 / iG2 talk to
     the mix directly.  Oracle: the portable 5-D block (reference semantics, dfno.py:82-97 with n = 3)."""
@@ -278,6 +277,27 @@ def test_memory_plan_sizes_shards_for_a_b200():
     assert HBM_BUDGET < 80 * 2 ** 30                                    # an H100 holds 80 GB
 
 
+def test_plan_routes_follow_the_shape_and_size_the_memory_check():
+    """The plan's route flags for every shape of the GPU route matrix, and supports() checking the memory of the route
+    that runs: at modes_z = 34 (2*KZ = 136 > 128) the round-1 dataflow also holds the channels-last head buffers and
+    dhb, which take this problem over the budget; at modes_z = 32 the fused pointwise dataflow fits."""
+    from dfno_b200.models.fused import HBM_BUDGET, _as_6d, supports
+    from test_spectral_conv_gpu import ROUTES
+    for name, in_shape, T, C, modes, routes in ROUTES:
+        _, (B, Cin, X, Y, Z, Tin), modes6, _ = _as_6d([1] * len(in_shape), in_shape, modes)
+        pl = EnginePlan(B, Cin, Tin, C, T, X, Y, Z, modes6)
+        assert (pl.fused_pw, pl.tc_bypass) == (routes["fused_pw"], routes["tc"]), name
+    g = _Grid(1, 1, 1, 1, 1, 1)
+    ok, why = supports(g, [1, 1, 256, 256, 72, 1], 20, 20, (12, 12, 34, 10))
+    assert not ok and "GiB per GPU" in why, why
+    pl = EnginePlan(1, 1, 1, 20, 20, 256, 256, 72, (12, 12, 34, 10))
+    pl.finish(4)
+    assert not pl.fused_pw and pl.memory_bytes()["total"] > HBM_BUDGET                  # 77.4 GiB
+    pl.fused_pw = True
+    assert pl.memory_bytes()["total"] < HBM_BUDGET                                      # 68.9 GiB
+    assert supports(g, [1, 1, 256, 256, 72, 1], 20, 20, (12, 12, 32, 10))[0]           # fused route, 67.0 GiB
+
+
 def test_column_parts_address_the_same_elements():
     """``ScatterSpec.column_part``: pair ``j`` of a part lands exactly where pair ``j0 + j`` of the whole
     stage does (same peer after slicing the peer table, same element offset), for row-, column- and
@@ -316,13 +336,15 @@ def test_cost_model_reproduces_measured_dram_traffic():
     to the dataflow; the tolerance (8 %, 12 % for spectral_out) covers that device's L2 hits."""
     pl = EnginePlan(1, 1, 1, 20, 20, 128, 128, 128, (12, 12, 12, 10), world=1, rank=0)
     pl.finish(4)
-    cm = pl.cost_model(legacy=True)
+    pl.fused_pw = False                                    # round-1 dataflow, which these counts were recorded on
+    cm = pl.cost_model()
     got = {n: b / 1e9 for n, _, b, _ in cm["stages"]}
     measured_gb = {"G1a": 2.27, "G1b": 0.91, "G2": 0.35, "iG1b": 0.96, "bypass fwd": 6.66, "bypass bwd": 8.35,
                    "spectral_mix fwd": 0.46, "spectral_mix bwd": 0.87, "adam": 12.3, "head fwd": 2.2, "head bwd": 4.2}
     for k, v in measured_gb.items():
         assert abs(got[k] - v) / v < 0.08, (k, got[k], v)
     assert 130e9 < cm["hbm_bytes"] < 175e9 and cm["nvlink_bytes"] == 0
+    pl.fused_pw = True
     cm = pl.cost_model()                                   # round-2 dataflow: fused pointwise kernels
     got = {n: b / 1e9 for n, _, b, _ in cm["stages"]}
     measured_gb = {"G1a": 2.274, "G1b": 0.910, "G2": 0.354, "iG1b": 0.952, "spectral_out fwd": 5.624, "dpre_dw": 6.852,

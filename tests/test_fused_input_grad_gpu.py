@@ -17,33 +17,31 @@ pytestmark = pytest.mark.gpu
 
 # Bounds, measured on an H100 80GB HBM3 over seeds 0, 1, 2 and set at about 4x the worst value seen (in brackets).
 # The worst case is large_mz (legacy route, tensor-core bypass) at seed 1; every other case stays at or below
-# 1.9e-2 / 0.10.
+# 1.9e-2 / 0.11 (legacy_t30: 1.3e-2 / 0.107).
 FRO = 9e-2          # relative Frobenius error of dx                                      [2.16e-2]
 POS = 0.95          # worst |dx - ref| at one position over the rms of ref                  [0.232]
 
-# (id, public in_shape, T, C, modes, expected fused_pw, DFNO_POINTWISE)
+# (id, public in_shape, T, C, modes, expected fused_pw)
 CASES = [
-    ("cin1_tin1", [1, 1, 16, 16, 16, 1], 8, 8, (4, 4, 4, 3), True, None),
-    ("cin2_tin3", [2, 2, 12, 8, 24, 3], 12, 20, (2, 4, 6, 7), True, None),
-    ("cin3_tin10", [1, 3, 16, 8, 16, 10], 40, 12, (2, 2, 4, 4), True, None),
-    ("cin4_tin1_c32", [1, 4, 16, 8, 16, 1], 8, 32, (2, 2, 4, 4), True, None),
-    ("lift_budget", [1, 1, 8, 8, 16, 64], 62, 8, (2, 2, 4, 4), True, None),   # test_spectral_conv_gpu.ROUTES
-    ("cin4_tin64", [1, 4, 8, 8, 16, 64], 60, 8, (2, 2, 4, 4), True, None),
-    ("t30_padded_pitch", [1, 2, 12, 12, 16, 1], 30, 20, (4, 4, 4, 8), True, None),
-    ("2d_time", [2, 1, 32, 32, 10], 16, 20, (4, 4, 4), True, None),
-    ("large_mz", [2, 1, 8, 8, 128, 1], 8, 12, (2, 2, 34, 3), False, None),   # legacy route, tensor-core bypass
-    ("2d_time_cuda_core", [2, 1, 12, 72, 1], 2, 16, (4, 34, 2), False, None),  # legacy route, CUDA-core bypass
-    ("legacy_env", [1, 2, 12, 12, 16, 1], 30, 20, (4, 4, 4, 8), False, "legacy"),
+    ("cin1_tin1", [1, 1, 16, 16, 16, 1], 8, 8, (4, 4, 4, 3), True),
+    ("cin2_tin3", [2, 2, 12, 8, 24, 3], 12, 20, (2, 4, 6, 7), True),
+    ("cin3_tin10", [1, 3, 16, 8, 16, 10], 40, 12, (2, 2, 4, 4), True),
+    ("cin4_tin1_c32", [1, 4, 16, 8, 16, 1], 8, 32, (2, 2, 4, 4), True),
+    ("lift_budget", [1, 1, 8, 8, 16, 64], 62, 8, (2, 2, 4, 4), True),   # test_spectral_conv_gpu.ROUTES
+    ("cin4_tin64", [1, 4, 8, 8, 16, 64], 60, 8, (2, 2, 4, 4), True),
+    ("t30_padded_pitch", [1, 2, 12, 12, 16, 1], 30, 20, (4, 4, 4, 8), True),
+    ("2d_time", [2, 1, 32, 32, 10], 16, 20, (4, 4, 4), True),
+    ("large_mz", [2, 1, 8, 8, 128, 1], 8, 12, (2, 2, 34, 3), False),   # legacy route, tensor-core bypass
+    ("2d_time_cuda_core", [2, 1, 12, 72, 1], 2, 16, (4, 34, 2), False),  # legacy route, CUDA-core bypass
+    ("legacy_t30", [1, 2, 8, 8, 72, 1], 30, 20, (2, 2, 34, 8), False),  # legacy route, padded t pitch (Tp = 32)
 ]
 CASE = {c[0]: c for c in CASES}
 
 
-def _models(case, monkeypatch, seed=0, blocks=2, ref_dtype=torch.float64):
+def _models(case, seed=0, blocks=2, ref_dtype=torch.float64):
     import dfno_b200 as d
     from dfno_b200.models.fused import FusedDistributedFNO
-    name, in_shape, T, C, modes, fused_pw, env = case
-    if env:
-        monkeypatch.setenv("DFNO_POINTWISE", env)
+    name, in_shape, T, C, modes, fused_pw = case
     _, P_x, _ = d.create_standard_partitions([1] * len(in_shape))
     dev = torch.device("cuda")
     torch.manual_seed(seed)
@@ -103,8 +101,8 @@ def passes(dx, ref, fro=FRO, pos=POS):
 # ------------------------------------------------------------------------------------------------ dx vs float64
 @pytest.mark.parametrize("seed", [0, 1, 2])
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
-def test_input_gradient_matches_float64(case, seed, monkeypatch):
-    d, ref, fused = _models(case, monkeypatch, seed=seed)
+def test_input_gradient_matches_float64(case, seed):
+    d, ref, fused = _models(case, seed=seed)
     x, w = _inputs(case, seed)
     dx = _dx(fused, x, w)
     assert dx.shape == x.shape and dx.dtype == x.dtype
@@ -116,10 +114,10 @@ def test_input_gradient_matches_float64(case, seed, monkeypatch):
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float64], ids=["bf16", "fp64"])
 @pytest.mark.parametrize("name", ["cin1_tin1", "cin3_tin10", "2d_time"])
-def test_input_gradient_in_the_input_dtype(name, dtype, monkeypatch):
+def test_input_gradient_in_the_input_dtype(name, dtype):
     """bf16 inputs are read as bf16 by the lift; fp64 inputs run as fp32.  dx comes back in the input's dtype."""
     case = CASE[name]
-    d, ref, fused = _models(case, monkeypatch)
+    d, ref, fused = _models(case)
     x, w = _inputs(case, 0, dtype)
     dx = _dx(fused, x, w)
     assert dx.dtype == dtype and dx.shape == x.shape
@@ -128,10 +126,10 @@ def test_input_gradient_in_the_input_dtype(name, dtype, monkeypatch):
     assert f < FRO and p < POS, (name, dtype, f, p)
 
 
-def test_the_checker_fails_on_a_wrong_input_gradient(monkeypatch):
+def test_the_checker_fails_on_a_wrong_input_gradient():
     """One input channel of dx zeroed, and one t term (of T = 40) dropped from the reference, are both rejected."""
     case = CASE["cin3_tin10"]
-    d, ref, fused = _models(case, monkeypatch)
+    d, ref, fused = _models(case)
     x, w = _inputs(case, 0)
     dx = _dx(fused, x, w)
     want = _ref_dx(ref, x, w)
@@ -147,9 +145,9 @@ def test_the_checker_fails_on_a_wrong_input_gradient(monkeypatch):
 
 # ------------------------------------------------------------------------------------------------ theta
 @pytest.mark.parametrize("name", ["cin2_tin3", "large_mz", "2d_time_cuda_core"])
-def test_input_gradient_leaves_the_weight_gradients_alone(name, monkeypatch):
+def test_input_gradient_leaves_the_weight_gradients_alone(name):
     case = CASE[name]
-    d, ref, fused = _models(case, monkeypatch)
+    d, ref, fused = _models(case)
     x, w = _inputs(case, 0)
     (fused(x) * w).sum().backward()
     g0 = fused.theta.grad.clone()
@@ -162,11 +160,11 @@ def test_input_gradient_leaves_the_weight_gradients_alone(name, monkeypatch):
 
 
 @pytest.mark.parametrize("name", ["cin2_tin3", "cin3_tin10", "large_mz", "2d_time_cuda_core"])
-def test_frozen_weights_give_dx_only(name, monkeypatch):
+def test_frozen_weights_give_dx_only(name):
     """theta.requires_grad_(False): theta.grad stays None, or bitwise equal to what a training backward left there,
     and dx is bitwise equal to the dx of a trainable theta (nothing on the dx path is atomic)."""
     case = CASE[name]
-    d, ref, fused = _models(case, monkeypatch)
+    d, ref, fused = _models(case)
     x, w = _inputs(case, 0)
     fused.theta.requires_grad_(False)
     dx_frozen = _dx(fused, x, w)
@@ -183,9 +181,9 @@ def test_frozen_weights_give_dx_only(name, monkeypatch):
     assert passes(dx_frozen, _ref_dx(ref, x, w))
 
 
-def test_double_backward_raises(monkeypatch):
+def test_double_backward_raises():
     case = CASE["cin1_tin1"]
-    d, ref, fused = _models(case, monkeypatch)
+    d, ref, fused = _models(case)
     x, w = _inputs(case, 0)
     xx = x.clone().requires_grad_()
     with pytest.raises(RuntimeError, match="double backward"):
@@ -202,15 +200,15 @@ def test_default_engine_still_refuses_input_gradients():
 
 
 # ------------------------------------------------------------------------------------------------ inversion
-def test_inversion_descends_and_tracks_the_fp32_backend(monkeypatch):
+def test_inversion_descends_and_tracks_the_fp32_backend():
     """Surrogate inversion: freeze the network and run Adam on its input towards y* = f(x*), where f is the network
     being inverted.  The loss of the frozen bf16 engine must fall >= 5x and track the same descent on the fp32
     portable backend within 10 %.  The comparison covers the first 40 steps (1.36 -> ~0.04): below a relative loss
     of about 2e-2, the bf16 activations' resolution, the engine's descent stalls while fp32 goes on (measured on an
     H100: 0.0205 against 0.0090 after 200 steps)."""
     import dfno_b200 as d
-    case = ("inv", [2, 1, 16, 16, 16, 1], 8, 12, (4, 4, 4, 3), True, None)
-    _, ref, fused = _models(case, monkeypatch, seed=11, ref_dtype=torch.float32)
+    case = ("inv", [2, 1, 16, 16, 16, 1], 8, 12, (4, 4, 4, 3), True)
+    _, ref, fused = _models(case, seed=11, ref_dtype=torch.float32)
     for p in ref.parameters():
         p.requires_grad_(False)
     fused.theta.requires_grad_(False)

@@ -64,10 +64,9 @@ def main():
            " (no measured NVLink rate)"))
     for name, calls, hb, lb in cm["stages"]:
         print(f"  {name:18s} x{calls:<3d} {hb / 1e9:8.3f} GB/call" + (f"  + {lb / 1e6:7.1f} MB NVLink" if lb else ""))
-    staged = P >= 8
-    print(f"\nstage chain ({'staged' if staged else 'direct'} peer layout), one spectral convolution"
+    print(f"\nstage chain ({'staged' if pl.staged else 'direct'} peer layout), one spectral convolution"
           " (G1a + G1b run as ONE kernel, spectral_in, when the shape allows: T <= 64, local Y % 4 == 0):")
-    for st in pl.chain(staged=staged):
+    for st in pl.chain(staged=pl.staged):
         if "N" not in st:
             print(f"  {st['name']:7s} {'local permutation ' + st['src'] + ' -> ' + st['dst'] if st['name'].startswith('perm') else 'per-mode channel mixing'}")
             continue
