@@ -108,5 +108,14 @@ const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const
                       long long n_dout, unsigned* amax_ws, void* g, float* gW3, float* gb3, float* gW4, float* gb4,
                       int B, int C, long long S, int nrl, const int* R, const long long* SR, int num_sms,
                       cudaStream_t stream);
+// projection head with O = 1..4 output channels (head_multi_sm90.cu): output channel o of a row at + o*plane.
+// w4b4 = [W4 (O x 128), b4 (O)]; the backward takes C <= 31 and reduces |dout| over all n_dout elements.
+const char* head_fwd_multi(const void* h, const void* W3aug, const float* w4b4, float* out, int B, int C, long long S,
+                           int O, long long plane, int nrl, const int* R, const long long* SR, int num_sms,
+                           cudaStream_t stream);
+const char* head_bwd_multi(const void* h, const void* W3aug, const void* W3T16, const float* W4, const float* dout,
+                           long long n_dout, unsigned* amax_ws, void* g, float* gW3, float* gb3, float* gW4, float* gb4,
+                           int B, int C, long long S, int O, long long plane, int nrl, const int* R,
+                           const long long* SR, int num_sms, cudaStream_t stream);
 
 }  // namespace dfno

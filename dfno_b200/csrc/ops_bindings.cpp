@@ -327,6 +327,43 @@ void head_bwd2(const at::Tensor& h, const at::Tensor& W3aug, const at::Tensor& W
                         static_cast<int>(radices.size()), R, SR, sm_count(), cur_stream()), "head_bwd2");
 }
 
+// out: fp32 [B, O, ...] addressed through the row digits, output channel o at + o * plane
+void head_fwd_multi(const at::Tensor& h, const at::Tensor& W3aug, const at::Tensor& w4b4, at::Tensor& out, int64_t B,
+                    int64_t C, int64_t S, int64_t O, int64_t plane, const std::vector<int64_t>& radices,
+                    const std::vector<int64_t>& strides) {
+  TORCH_CHECK(radices.size() == strides.size() && !radices.empty() && radices.size() <= 4, "1..4 row digits");
+  TORCH_CHECK(W3aug.dim() == 2 && W3aug.size(0) == 128 && W3aug.size(1) == 64 && W3aug.is_contiguous(), "W3aug [128,64]");
+  TORCH_CHECK(w4b4.numel() >= O * 129, "w4b4 = [W4 (O x 128), b4 (O)]");
+  TORCH_CHECK(out.numel() >= B * O * S, "out smaller than B * O * S");
+  c10::cuda::CUDAGuard guard(h.device());
+  int R[4]; long long SR[4];
+  for (size_t i = 0; i < 4; ++i) { R[i] = i < radices.size() ? static_cast<int>(radices[i]) : 1; SR[i] = i < strides.size() ? strides[i] : 0; }
+  check(dfno::head_fwd_multi(bptr(h), bptr(W3aug), fptr(w4b4), fptr_mut(out), static_cast<int>(B), static_cast<int>(C),
+                             S, static_cast<int>(O), plane, static_cast<int>(radices.size()), R, SR, sm_count(),
+                             cur_stream()), "head_fwd_multi");
+}
+
+void head_bwd_multi(const at::Tensor& h, const at::Tensor& W3aug, const at::Tensor& W3T16, const at::Tensor& W4,
+                    const at::Tensor& dout, at::Tensor& amax_ws, at::Tensor& g, at::Tensor& gW3, at::Tensor& gb3,
+                    at::Tensor& gW4, at::Tensor& gb4, int64_t B, int64_t C, int64_t S, int64_t O, int64_t plane,
+                    const std::vector<int64_t>& radices, const std::vector<int64_t>& strides) {
+  TORCH_CHECK(radices.size() == strides.size() && !radices.empty() && radices.size() <= 4, "1..4 row digits");
+  TORCH_CHECK(W3aug.dim() == 2 && W3aug.size(0) == 128 && W3aug.size(1) == 64 && W3aug.is_contiguous(), "W3aug [128,64]");
+  TORCH_CHECK(W3T16.is_cuda() && W3T16.scalar_type() == at::kHalf && W3T16.dim() == 2 && W3T16.size(1) == 128 &&
+              W3T16.size(0) == (C + 1 + 15) / 16 * 16 && W3T16.is_contiguous(), "W3T16: fp16 [ceil16(C+1), 128]");
+  TORCH_CHECK(W4.numel() == O * 128 && gW4.numel() == O * 128 && gb4.numel() == O, "W4 / dW4 [O, 128], db4 [O]");
+  TORCH_CHECK(dout.numel() >= B * O * S, "dout smaller than B * O * S");
+  TORCH_CHECK(amax_ws.is_cuda() && amax_ws.numel() >= 1 && amax_ws.element_size() == 4, "amax_ws: one 32-bit word");
+  c10::cuda::CUDAGuard guard(h.device());
+  int R[4]; long long SR[4];
+  for (size_t i = 0; i < 4; ++i) { R[i] = i < radices.size() ? static_cast<int>(radices[i]) : 1; SR[i] = i < strides.size() ? strides[i] : 0; }
+  check(dfno::head_bwd_multi(bptr(h), bptr(W3aug), W3T16.data_ptr(), fptr(W4), fptr(dout), dout.numel(),
+                             reinterpret_cast<unsigned*>(amax_ws.data_ptr()), bptr(g), fptr_mut(gW3), fptr_mut(gb3),
+                             fptr_mut(gW4), fptr_mut(gb4), static_cast<int>(B), static_cast<int>(C), S,
+                             static_cast<int>(O), plane, static_cast<int>(radices.size()), R, SR, sm_count(),
+                             cur_stream()), "head_bwd_multi");
+}
+
 }  // namespace
 
 void register_ops(pybind11::module& m) {
@@ -340,6 +377,8 @@ void register_ops(pybind11::module& m) {
   m.def("dpre_dw", &dpre_dw);
   m.def("head_fwd", &head_fwd);
   m.def("head_bwd2", &head_bwd2);
+  m.def("head_fwd_multi", &head_fwd_multi);
+  m.def("head_bwd_multi", &head_bwd_multi);
   m.def("lift_fwd", &lift_fwd);
   m.def("lift_bwd", &lift_bwd, py::arg("x"), py::arg("W1"), py::arg("b1"), py::arg("W2"), py::arg("b2"), py::arg("dh"),
         py::arg("gW1"), py::arg("gb1"), py::arg("gW2"), py::arg("gb2"), py::arg("dims"), py::arg("dx") = c10::nullopt);

@@ -282,6 +282,15 @@ __device__ __forceinline__ void wg_mma64(float (&acc)[R], int n, uint64_t da, ui
 #undef DFNO_WG_CASE
 #undef DFNO_WG_CASE16
 
+// m64n8k16, fp16 inputs, both operands from shared memory: d = the 4 accumulator registers of an m64n8 tile
+template <int kTA, int kTB>
+__device__ __forceinline__ void wgmma_m64n8k16_f16(float (&d)[4], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %6, 0;\nwgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 "
+               "{%0,%1,%2,%3}, %4, %5, p, 1, 1, %7, %8;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "l"(da), "l"(db), "r"(scale_d), "n"(kTA), "n"(kTB));
+}
+
 // One k16 step of a 128 x n tile (n <= R): rows 0..63 into acc[0, R/2), rows 64..127 into acc[R/2, R).
 // `a_half_bytes` is the step to the second half of A (8192 B for a K-major block, LBO for an MN-major one).
 template <bool kF16, int TA, int TB, int R>

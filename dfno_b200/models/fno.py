@@ -253,14 +253,15 @@ class DistributedFNOBlock(nn.Module):
 
 class DistributedFNO(nn.Module):
     """Lift (time axis ``T_in->T_out``, channels ``C_in->width``), ``num_blocks`` Fourier
-    layers, projection ``width->128->1``.  ``in_shape`` is the **global**
+    layers, projection ``width->128->out_channels``.  ``in_shape`` is the **global**
     ``[B, C_in, *spatial, T_in]``; the forward takes/returns this rank's ``P_x`` shard
     (reference ``dfno/dfno.py:293-353``).
 
     ``backend="auto"`` hands construction to the fused sm_90a engine when the device,
     dtype and partition are ones it covers (see :func:`dfno_b200.models.fused.supports`);
     ``backend="torch"`` forces this portable implementation.  ``input_grad=True`` asks for dL/dx on either backend
-    (the fused engine refuses an input that requires grad without it).
+    (the fused engine refuses an input that requires grad without it).  ``out_channels`` (default 1) predicts that
+    many fields from one trunk: the output is ``[B, out_channels, *spatial, T_out]``.
     """
 
     def __new__(cls, *args, backend: str = "auto", **kwargs):
@@ -273,10 +274,12 @@ class DistributedFNO(nn.Module):
     def __init__(self, P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width: int,
                  modes: Sequence[int], num_blocks: int = 4, device=torch.device("cpu"),
                  dtype=torch.float32, plan: str = "reference", backend: str = "auto",
-                 init_seed: Optional[int] = None, fft_impl: str = "torch", input_grad: bool = False):
+                 init_seed: Optional[int] = None, fft_impl: str = "torch", input_grad: bool = False,
+                 out_channels: int = 1):
         # input_grad: accepted for constructor parity with the fused engine (which returns dL/dx only when asked);
         # this backend always differentiates its input
         super().__init__()
+        self.out_channels = check_out_channels(out_channels)
         if init_seed is not None:       # reproducible draw (per rank; the fused engine's is partition independent)
             torch.manual_seed(int(init_seed) + 7919 * max(int(P_x.rank), 0))
         self.P_x = P_x
@@ -303,7 +306,7 @@ class DistributedFNO(nn.Module):
             work[tgt] *= extra
             if work[tgt] > self.in_shape[tgt]:
                 raise ValueError(f"cannot fold {extra} time/channel workers onto a spatial axis of {self.in_shape}")
-            out_shape = [self.in_shape[0], 1, *self.in_shape[2:-1], self.out_timesteps]
+            out_shape = [self.in_shape[0], self.out_channels, *self.in_shape[2:-1], self.out_timesteps]
             P_work = P_x.create_cartesian_topology_partition(work)
             self.R_in = Repartition(P_x, P_work, self.in_shape, dtype=dtype)
             self.R_out = Repartition(P_work, P_x, out_shape, dtype=dtype)
@@ -315,7 +318,7 @@ class DistributedFNO(nn.Module):
         self.linear1 = BroadcastedLinear(P_x, self.in_shape[-1], self.out_timesteps, dim=-1, **kw)
         self.linear2 = BroadcastedLinear(P_x, self.in_shape[1], self.width, dim=1, **kw)
         self.linear3 = BroadcastedLinear(P_x, self.width, 128, dim=1, **kw)
-        self.linear4 = BroadcastedLinear(P_x, 128, 1, dim=1, **kw)
+        self.linear4 = BroadcastedLinear(P_x, 128, self.out_channels, dim=1, **kw)
         self.blocks = nn.ModuleList(
             DistributedFNOBlock(P_x, self.block_in_shape, self.modes, plan=plan, fft_impl=fft_impl, **kw)
             for _ in range(self.num_blocks))
@@ -338,6 +341,13 @@ class DistributedFNO(nn.Module):
             x = self.R_out(x)
         self.dt_comm = dt
         return x
+
+
+def check_out_channels(out_channels) -> int:
+    """``out_channels`` as an int >= 1 (``ValueError`` otherwise)."""
+    if isinstance(out_channels, bool) or not isinstance(out_channels, (int, np.integer)) or int(out_channels) < 1:
+        raise ValueError(f"out_channels must be an integer >= 1, got {out_channels!r}")
+    return int(out_channels)
 
 
 def infer_global_shape(P: Partition, local_shape: Sequence[int]) -> List[int]:

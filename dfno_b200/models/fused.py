@@ -45,6 +45,7 @@ from ..parallel.partition import Partition
 __all__ = ["FusedDistributedFNO", "FusedAdam", "supports", "wants", "EnginePlan", "fold_onto_pencil"]
 
 SUPPORTED_WIDTHS = (4, 8, 12, 16, 20, 24, 32)
+MAX_OUT = 4                  # output channels of the multi-output head kernels (csrc/head_multi_sm90.cu)
 MAX_N = 256                  # n_pad limit of dft_gemm (accumulator columns of one 64-row warpgroup tile)
 HBM_BUDGET = 72 * 2 ** 30    # of an H100's 80 GB: leave room for the CUDA context, NCCL and the allocator
 HEAD_HIDDEN = 128
@@ -81,9 +82,10 @@ def _pencil_axis(grid: Sequence[int]) -> Optional[int]:
     return None
 
 
-def fold_onto_pencil(P_x: Partition, in_shape: Sequence[int], out_timesteps: int):
+def fold_onto_pencil(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, out_channels: int = 1):
     """``(P_work, R_in, R_out)``: the y-pencil over ``P_x``'s ranks and the two re-shards that move
-    the network input onto it and the output back (``None`` when ``P_x`` already is that pencil)."""
+    the network input onto it and the ``out_channels``-channel output back (``None`` when ``P_x`` already is that
+    pencil)."""
     if _pencil_axis(P_x.shape) is not None:
         return P_x, None, None
     from ..parallel.primitives import Repartition
@@ -91,20 +93,24 @@ def fold_onto_pencil(P_x: Partition, in_shape: Sequence[int], out_timesteps: int
     work = [1] * nd
     work[nd - 3] = int(np.prod(P_x.shape))
     P_work = P_x.create_cartesian_topology_partition(work)
-    out_shape = [int(in_shape[0]), 1, *[int(v) for v in in_shape[2:-1]], int(out_timesteps)]
+    out_shape = [int(in_shape[0]), int(out_channels), *[int(v) for v in in_shape[2:-1]], int(out_timesteps)]
     return P_work, Repartition(P_x, P_work, [int(v) for v in in_shape]), Repartition(P_work, P_x, out_shape)
 
 
 def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width: int,
-             modes: Sequence[int]) -> Tuple[bool, str]:
+             modes: Sequence[int], out_channels: int = 1) -> Tuple[bool, str]:
     """Can the fused engine run this configuration?  Returns ``(ok, reason)``.
 
     The engine computes on a ``(1,1,1,P,1,1)`` y-pencil.  Any other 6-D ``P_x`` without a batch
     split (e.g. BASELINE config 3's ``(1,1,2,2,2,1)`` or config 4's 8-way time partition) is served
     by re-sharding the (small) network input onto that pencil once, running the engine there and
-    re-sharding the single-channel output back -- instead of the reference's two full-resolution
+    re-sharding the output back -- instead of the reference's two full-resolution
     re-shards R1/R4 per Fourier layer (``dfno/dfno.py:247,288`` of the reference).  5-D (2-D + time)
-    problems run as 6-D ones with a singleton x axis (:func:`_as_6d`)."""
+    problems run as 6-D ones with a singleton x axis (:func:`_as_6d`).  ``out_channels`` > 1 (at most
+    :data:`MAX_OUT`) runs the multi-output head kernels, which exist on the round-2 route only.  An
+    ``out_channels`` that is not an integer >= 1 raises ``ValueError``."""
+    from .fno import check_out_channels
+    O = check_out_channels(out_channels)
     six = _as_6d(P_x.shape, in_shape, modes)
     if six is None:
         return False, "fused engine covers 2-D + time and 3-D + time fields (5-D / 6-D tensors)"
@@ -117,6 +123,14 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
     mx, my, mz, mt = modes6
     if width not in SUPPORTED_WIDTHS:
         return False, f"width {width} not in {SUPPORTED_WIDTHS}"
+    if O > MAX_OUT:
+        return False, f"out_channels = {O}: the fused projection head covers 1 <= out_channels <= {MAX_OUT}"
+    if O > 1 and 2 * (2 * mz) > 128:
+        return False, (f"out_channels = {O} needs the round-2 route (2 * 2 * modes_z <= 128, here {4 * mz}); the "
+                       f"round-1 head is single-output")
+    if O > 1 and width > 31:
+        return False, (f"out_channels = {O} at width {width}: the multi-output head backward covers width <= 31 "
+                       f"(its consumer registers run out at 32)")
     if P > 8:
         return False, "at most 8 peers (one NVSwitch box)"
     if Y % P or (2 * mz) % P:
@@ -137,7 +151,7 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
         return False, "transformed axes: Z <= 256, T <= 128, X, Y <= 256 samples"
     if B * width * X * (Y // P) * Z * T >= 2 ** 31:
         return False, "per-rank activation must stay below 2^31 elements"
-    pl = EnginePlan(B, Cin, Tin, width, T, X, Y, Z, modes6, world=P, rank=0)
+    pl = EnginePlan(B, Cin, Tin, width, T, X, Y, Z, modes6, world=P, rank=0, out_channels=O)
     pl.finish(4)
     need = pl.memory_bytes(train=True)["total"]
     if need > HBM_BUDGET:
@@ -174,7 +188,8 @@ def wants(args, kwargs, backend: str) -> bool:
     device = torch.device(cfg.get("device", "cpu"))
     dtype = cfg.get("dtype", torch.float32)
     try:
-        ok, why = supports(cfg["P_x"], cfg["in_shape"], cfg["out_timesteps"], cfg["width"], cfg["modes"])
+        ok, why = supports(cfg["P_x"], cfg["in_shape"], cfg["out_timesteps"], cfg["width"], cfg["modes"],
+                           out_channels=cfg.get("out_channels", 1))
     except Exception as e:           # noqa: BLE001 - malformed arguments: let the portable constructor report them
         ok, why = False, f"{type(e).__name__}: {e}"
     if backend == "fused":
@@ -193,8 +208,9 @@ def wants(args, kwargs, backend: str) -> bool:
 class EnginePlan:
     """All integer bookkeeping of one rank; no tensors, no CUDA -- unit-testable on CPU."""
 
-    def __init__(self, B, Cin, Tin, C, T, X, Y, Z, modes, world=1, rank=0, hidden=HEAD_HIDDEN):
+    def __init__(self, B, Cin, Tin, C, T, X, Y, Z, modes, world=1, rank=0, hidden=HEAD_HIDDEN, out_channels=1):
         self.B, self.Cin, self.Tin, self.C, self.T = B, Cin, Tin, C, T
+        self.O = int(out_channels)                         # output channels (fields) of the head
         self.X, self.Y, self.Z = X, Y, Z
         self.mx, self.my, self.mz, self.mt = [int(m) for m in modes]
         self.world, self.rank, self.H = world, rank, hidden
@@ -255,7 +271,7 @@ class EnginePlan:
         for k in range(num_blocks):
             seg(f"blocks.{k}.linear.W", C, C)
         seg("linear3.W", H, C); seg("linear3.b", H)
-        seg("linear4.W", 1, H); seg("linear4.b", 1)
+        seg("linear4.W", self.O, H); seg("linear4.b", self.O)          # adjacent: FusedDistributedFNO._w4b4
         self.n_small = (off + 63) // 64 * 64               # replicated segment (all-reduced)
         off = self.n_small
         for k in range(num_blocks):
@@ -374,7 +390,7 @@ class EnginePlan:
             "workspaces": (max(self.n_Z1, self.n_U) + self.n_S1 + self.n_T1 + self.n_S2 + 2 * self.n_S3 + self.n_T2) * bf,
             "staging": (((self.n_S1 + self.n_T1) * bf if self.staged else 0) + self.n_small * f32
                         if self.world > 1 else 0),
-            "input_output": self.B * self.S // self.T * self.Cin * self.Tin * f32 + self.B * self.S * f32,
+            "input_output": self.B * self.S // self.T * self.Cin * self.Tin * f32 + self.O * self.B * self.S * f32,
         }
         if train and legacy:            # round-1 dataflow: channels-last head, separate bypass
             out["saved_activations"] = (2 * nb * self.n_act + nb * self.n_S3 + cl) * bf
@@ -428,13 +444,14 @@ class EnginePlan:
                ("lift fwd", 1, act, 0), ("lift bwd", 1, act, 0), ("adam", 1, 7 * self.n_theta * f32, 0)]
         if legacy:
             st += [("iG1a add (bwd)", nb, act, 0), ("bypass fwd", nb, 4 * act, 0), ("bypass bwd", nb, 5 * act, 0),
-                   ("head fwd", 1, cl + self.npos * f32, 0), ("head bwd", 1, 2 * cl + self.npos * f32, 0)]
+                   ("head fwd", 1, cl + self.O * self.npos * f32, 0), ("head bwd", 1, 2 * cl + self.O * self.npos * f32, 0)]
         else:
             # the chain's last GEMM also applies the bypass conv (+ GELU): reads U and the block input, writes the
             # pre-activation and the output (forward) / reads U and dpre, writes the input gradient (adjoint)
             st += [("spectral_out fwd", nb, U + 3 * act, 0), ("spectral_out adj", nb, U + 2 * act, 0),
                    ("dpre_dw", nb, 4 * act, 0),
-                   ("head fwd", 1, act + self.npos * f32, 0), ("head bwd", 1, 2 * act + 2 * self.npos * f32, 0)]
+                   ("head fwd", 1, act + self.O * self.npos * f32, 0),
+                   ("head bwd", 1, 2 * act + 2 * self.O * self.npos * f32, 0)]
         hbm = sum(c * b for _, c, b, _ in st)
         link = sum(c * l for _, c, _, l in st)
         return {"stages": st, "hbm_bytes": hbm, "nvlink_bytes": link,
@@ -545,7 +562,7 @@ class _FusedFn(torch.autograd.Function):
 class FusedDistributedFNO(nn.Module):
     """Drop-in ``DistributedFNO`` on the fused sm_90a engine.  Same constructor; the forward
     takes this rank's ``[B, C_in, X, Y_local, Z, T_in]`` shard (fp32 or bf16, CUDA) and returns
-    ``[B, 1, X, Y_local, Z, T_out]`` in fp32.
+    ``[B, out_channels, X, Y_local, Z, T_out]`` in fp32.
 
     ``input_grad=True``: an input that requires grad gets dL/dx (in its own dtype and shape) from the backward, for
     surrogate inversion and sensitivity studies.  With ``theta.requires_grad_(False)`` that backward computes dL/dx
@@ -554,10 +571,11 @@ class FusedDistributedFNO(nn.Module):
     def __init__(self, P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width: int,
                  modes: Sequence[int], num_blocks: int = 4, device=torch.device("cuda"),
                  dtype=torch.bfloat16, plan: Optional[str] = None, backend: str = "fused",
-                 use_p2p: Optional[bool] = None, init_seed: Optional[int] = None, input_grad: bool = False):
+                 use_p2p: Optional[bool] = None, init_seed: Optional[int] = None, input_grad: bool = False,
+                 out_channels: int = 1):
         super().__init__()
         self.input_grad = bool(input_grad)
-        ok, why = supports(P_x, in_shape, out_timesteps, width, modes)
+        ok, why = supports(P_x, in_shape, out_timesteps, width, modes, out_channels=out_channels)
         if not ok:
             raise ValueError(f"fused engine cannot run this configuration: {why}")
         from ..ops import build
@@ -567,6 +585,7 @@ class FusedDistributedFNO(nn.Module):
         self.out_timesteps, self.width = int(out_timesteps), int(width)
         self.modes = [int(m) for m in modes]
         self.num_blocks = int(num_blocks)
+        self.out_channels = int(out_channels)
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise ValueError("the fused engine needs a CUDA device")
@@ -580,13 +599,13 @@ class FusedDistributedFNO(nn.Module):
         # work partition: the y-pencil the engine computes on.  A differently shaped P_x is folded
         # onto it once at the network's entry / exit (see supports()).
         self.P_outer = P_x
-        self.P_work, self.R_in, self.R_out = fold_onto_pencil(P_x, self.in_shape, self.out_timesteps)
+        self.P_work, self.R_in, self.R_out = fold_onto_pencil(P_x, self.in_shape, self.out_timesteps, self.out_channels)
         P_x = self.P_work
         pa = P_x.dim - 3                             # the pencil axis of the work partition
         self.world = int(P_x.shape[pa]) if P_x.active else 1
         self.rank = int(P_x.index[pa]) if P_x.active else 0
         self.plan = EnginePlan(B, Cin, Tin, self.width, self.out_timesteps, X, Y, Z, modes6,
-                               self.world, self.rank)
+                               self.world, self.rank, out_channels=self.out_channels)
         self.plan.finish(self.num_blocks)
         pl = self.plan
         self.dt_comm = 0.0
@@ -860,16 +879,20 @@ class FusedDistributedFNO(nn.Module):
         return out
 
     def _w4b4(self) -> torch.Tensor:
-        """``[W4 (H), b4 (1)]`` -- adjacent in the flat parameter buffer by construction."""
-        off, _ = self.plan.segments["linear4.W"]
-        assert self.plan.segments["linear4.b"][0] == off + self.plan.H
-        return self.theta.data[off:off + self.plan.H + 1]
+        """``[W4 (O x H), b4 (O)]`` -- adjacent in the flat parameter buffer by construction."""
+        pl = self.plan
+        off, _ = pl.segments["linear4.W"]
+        assert pl.segments["linear4.b"][0] == off + pl.O * pl.H
+        return self.theta.data[off:off + pl.O * (pl.H + 1)]
 
     def _head_row_digits(self):
         """Row (b, x, y, t, z) of the engine layout -> element offset in the public
-        ``[B, 1, X, Y, Z, T]`` output: digits innermost first."""
+        ``[B, O, X, Y, Z, T]`` output: digits innermost first.  With several output channels the batch index is its
+        own digit (stride O*S) and channel o sits at + o*S (the plane stride)."""
         pl = self.plan
-        return [pl.Z, pl.T, pl.B * pl.X * pl.Yl], [pl.T, 1, pl.Z * pl.T]
+        if pl.O == 1:
+            return [pl.Z, pl.T, pl.B * pl.X * pl.Yl], [pl.T, 1, pl.Z * pl.T]
+        return [pl.Z, pl.T, pl.X * pl.Yl, pl.B], [pl.T, 1, pl.Z * pl.T, pl.O * pl.S]
 
     def _head_forward(self, hcl: torch.Tensor) -> torch.Tensor:
         """linear3 -> gelu -> linear4 in the epilogue of one wgmma GEMM (EPI_HEAD)."""
@@ -929,9 +952,12 @@ class FusedDistributedFNO(nn.Module):
                                                    pre=pres[k] if save else None))
             with _nvtx("dfno.head"):
                 w3a, _ = self._head_operators_cm()
-                out = torch.empty(pl.B, 1, pl.X, pl.Yl, pl.Z, pl.T, device=self.device, dtype=torch.float32)
+                out = torch.empty(pl.B, pl.O, pl.X, pl.Yl, pl.Z, pl.T, device=self.device, dtype=torch.float32)
                 R, SR = self._head_row_digits()
-                C_.head_fwd(hs[nb], w3a, self._w4b4(), out, pl.B, pl.C, pl.S, R, SR)
+                if pl.O == 1:
+                    C_.head_fwd(hs[nb], w3a, self._w4b4(), out, pl.B, pl.C, pl.S, R, SR)
+                else:
+                    C_.head_fwd_multi(hs[nb], w3a, self._w4b4(), out, pl.B, pl.C, pl.S, pl.O, pl.S, R, SR)
                 return out.squeeze(2) if self.five_d else out
         hcl = self._saved["hcl"]
         for k in range(nb):
@@ -984,9 +1010,14 @@ class FusedDistributedFNO(nn.Module):
             with _nvtx("dfno.head.bwd"):
                 w3a, w3t = self._head_operators_cm()
                 R, SR = self._head_row_digits()
-                C_.head_bwd2(hs[nb], w3a, w3t, self._seg("linear4.W").view(-1), dy.contiguous().float(),
-                             self.ws["amax"], g, self._seg("linear3.W", gf), self._seg("linear3.b", gf),
-                             self._seg("linear4.W", gf).view(-1), self._seg("linear4.b", gf), pl.B, pl.C, pl.S, R, SR)
+                head_grads = (self._seg("linear3.W", gf), self._seg("linear3.b", gf),
+                              self._seg("linear4.W", gf).view(-1), self._seg("linear4.b", gf))
+                if pl.O == 1:
+                    C_.head_bwd2(hs[nb], w3a, w3t, self._seg("linear4.W").view(-1), dy.contiguous().float(),
+                                 self.ws["amax"], g, *head_grads, pl.B, pl.C, pl.S, R, SR)
+                else:
+                    C_.head_bwd_multi(hs[nb], w3a, w3t, self._seg("linear4.W").view(-1), dy.contiguous().float(),
+                                      self.ws["amax"], g, *head_grads, pl.B, pl.C, pl.S, pl.O, pl.S, R, SR)
             L = pl.X * pl.Yl * pl.T
             for k in reversed(range(nb)):
                 with _nvtx(f"dfno.block{k}.bwd"):
@@ -1070,7 +1101,7 @@ class FusedDistributedFNO(nn.Module):
         pl = self.plan
         return {"format": "fused-theta", "segments": dict(pl.segments), "C": pl.C, "kzl": pl.kzl, "kz_off": pl.kz_off,
                 "mt": pl.mt, "KX": pl.KX, "KY": pl.KY, "KZ": pl.KZ, "rank": self.rank, "world": self.world,
-                "num_blocks": self.num_blocks, "ndim": len(self.in_shape)}
+                "num_blocks": self.num_blocks, "ndim": len(self.in_shape), "out_channels": pl.O}
 
     @staticmethod
     def theta_to_canonical(theta: torch.Tensor, meta: Dict[str, object], include_pointwise: bool = True):
@@ -1150,6 +1181,9 @@ class FusedDistributedFNO(nn.Module):
                     w = torch.view_as_real(w.permute(0, 1, 4, 5, 3, 2).contiguous())   # [i,o,kzl,mt,KY,KX,2]
                     self._seg(name).copy_(w.reshape(shape).to(self.device))
                 else:
+                    if src.numel() != int(np.prod(shape)):
+                        raise ValueError(f"canonical state entry {name} has shape {list(src.shape)}, this engine needs "
+                                         f"{list(shape)} (out_channels = {pl.O})")
                     self._seg(name).copy_(src.reshape(shape).to(self.device, torch.float32))
 
 

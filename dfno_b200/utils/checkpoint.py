@@ -122,6 +122,9 @@ def load_global_state(model, state: Optional[Dict[str, torch.Tensor]], src_is_ro
         elif t.numel() == 0:
             new[name] = t
         elif name in state:
+            if state[name].numel() != t.numel():          # e.g. a checkpoint of a model with other out_channels
+                raise ValueError(f"canonical state entry {name} has shape {list(state[name].shape)}, the model "
+                                 f"needs {list(t.shape)}")
             new[name] = state[name].to(device=t.device, dtype=t.dtype).reshape(t.shape)
         elif strict:
             raise KeyError(name)

@@ -30,6 +30,7 @@ def main():
     ap.add_argument("--in-channels", type=int, default=1)
     ap.add_argument("--in-timesteps", type=int, default=1)
     ap.add_argument("--blocks", type=int, default=4)
+    ap.add_argument("--out-channels", type=int, default=1, help="fields predicted by the network (default 1)")
     ap.add_argument("--hbm-gbs", type=float, default=None,
                     help="HBM copy bandwidth for the traffic floor (default: the value measured on an H100)")
     ap.add_argument("--nvlink-gbs", type=float, default=None, help="measured peer-copy rate (default: not estimated)")
@@ -37,15 +38,17 @@ def main():
     X, Y, Z, T = a.shape
     grid = a.partition or [1, 1, 1, a.gpus, 1, 1]
     in_shape = [a.batch, a.in_channels, X, Y, Z, a.in_timesteps]
-    ok, why = supports(_Grid(grid), in_shape, T, a.width, a.modes)
-    print(f"P_x = {tuple(grid)}  in_shape = {in_shape}  T_out = {T}  width = {a.width}  modes = {tuple(a.modes)}")
+    ok, why = supports(_Grid(grid), in_shape, T, a.width, a.modes, out_channels=a.out_channels)
+    print(f"P_x = {tuple(grid)}  in_shape = {in_shape}  T_out = {T}  width = {a.width}  modes = {tuple(a.modes)}"
+          + (f"  out_channels = {a.out_channels}" if a.out_channels != 1 else ""))
     print(f"fused engine: {'yes' if ok else 'no -- ' + why}")
     P = 1
     for g in grid:
         P *= g
     if Y % P or (2 * a.modes[2]) % P:
         return 0 if ok else 1
-    pl = EnginePlan(a.batch, a.in_channels, a.in_timesteps, a.width, T, X, Y, Z, a.modes, world=P, rank=0)
+    pl = EnginePlan(a.batch, a.in_channels, a.in_timesteps, a.width, T, X, Y, Z, a.modes, world=P, rank=0,
+                    out_channels=a.out_channels)
     pl.finish(a.blocks)
     if tuple(grid) != (1, 1, 1, P, 1, 1):
         print(f"work partition: (1, 1, 1, {P}, 1, 1) (input / output re-sharded once per step)")
