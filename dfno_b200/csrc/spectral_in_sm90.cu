@@ -18,6 +18,8 @@
 //
 // Warp roles: 0 .. 4E-1 = E consumer warpgroups (MMA1, epi-1, MMA2, epi-2 of their tiles; warpgroup g owns tiles
 // i = g (mod E) and the A2 buffer of that slot), 4E = TMA producer, 4E+1 = store warp.
+#include <algorithm>
+
 #include "sm90_ptx.cuh"
 #include "kernels.h"
 #include "tma_host.h"
@@ -26,7 +28,11 @@ namespace dfno {
 namespace {
 
 constexpr int kMaxPeersIn = 8;
-constexpr int kMaxE = 2;                      // consumer warpgroups (accumulators of up to 128 registers each)
+// consumer warpgroups: two while the accumulator takes at most 64 registers, one beyond (two would spill)
+constexpr int max_groups(int acc_regs) { return acc_regs <= 64 ? 2 : 1; }
+// MMA2 widths beyond 80 (mt > 40, not an FNO truncation of T <= 64 steps) run as N = 128: the extra operator rows
+// the wgmma reads are never stored
+constexpr int mma2_width(int n2_pad) { return n2_pad <= 80 ? n2_pad : 128; }
 constexpr int kMaxStagesIn = 6;
 
 struct alignas(64) PeerMaps {
@@ -40,9 +46,11 @@ struct SpecInParams {
   int KZ, mt, kzl, P;
   int Yc, tpc, ncy;          // positions per chunk, tiles per chunk, chunks per row
   int k1blocks, n1_pad;      // operator 1: 64-wide K blocks, padded rows (= MMA1 N)
-  int k2blocks, n2_pad, k2steps;
+  int k2blocks, n2_pad;      // operator 2: 64-wide K blocks (MMA2 runs all of them), padded rows (= MMA2 N)
   int stages, E;
   uint32_t blk1, stage_bytes, a2blk, a2_bytes, stg_bytes, peer_bytes;
+  uint32_t smem_bytes;
+  uint32_t swz;              // staging swizzle: Yc / 4 - 1 (the 16-byte chunks of a 128-byte line that are XORed)
 };
 
 __device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1,
@@ -53,26 +61,52 @@ __device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, const void* s
                : "memory");
 }
 
-// D (+)= A . B^T over `ksteps` k16 steps, both operands K-major in 64-wide blocks (a_blk / b_blk bytes apart); the
-// second m64 half is skipped when the tile has at most 64 rows (its A rows would lie past the operand block).
-template <int R>
-__device__ __forceinline__ void mma_kmajor(float (&acc)[R], int n, int rows, uint32_t a, uint32_t a_blk, uint32_t b,
-                                           uint32_t b_blk, int ksteps) {
-  wgmma_fence();
-  for (int ks = 0; ks < ksteps; ++ks) {
-    const uint32_t kb = ks >> 2, kk = ks & 3;
-    const uint64_t da = gdesc_k128(a + kb * a_blk + kk * 32), db = gdesc_k128(b + kb * b_blk + kk * 32);
-    if (rows > 64) wg_mma128<false, 0, 0>(acc, n, da, 8192, db, ks > 0 ? 1u : 0u);
-    else wg_mma64<false, 0, 0, 0>(acc, n, da, db, ks > 0 ? 1u : 0u);
-  }
+// D = A . B^T over `kblocks` >= 1 K blocks of 64 (four k16 steps each), both operands K-major (a_blk / b_blk bytes
+// per block), N columns and kHalves m64 halves (rows 64..127 into acc[R/2, R)).  N and kHalves are compile-time
+// constants and the k16 steps of a block are unrolled, so that the chain's wgmmas issue back to back with one commit
+// and one wait: a width chosen per instruction makes ptxas serialise every wgmma (C7511), and a fully unrolled
+// K loop runs out of (uniform) registers for the descriptors and is serialised too.  The block loop is a run-time
+// loop with a fence per block; ptxas closes it with one extra arrive before the wait (C7519).
+template <int N, int kHalves, int R>
+__device__ __forceinline__ void mma_chain(float (&acc)[R], uint32_t a, uint32_t a_blk, uint32_t b, uint32_t b_blk,
+                                          int kblocks) {
+  int kb = 0;
+#pragma unroll 1
+  do {
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const uint64_t da = gdesc_k128(a + kb * a_blk + kk * 32), db = gdesc_k128(b + kb * b_blk + kk * 32);
+      const uint32_t scale_d = kb > 0 || kk > 0 ? 1u : 0u;
+      wg_mma64<false, 0, 0, 0>(acc, N, da, db, scale_d);
+      if constexpr (kHalves == 2) wg_mma64<false, 0, 0, R / 2>(acc, N, da + (8192 >> 4), db, scale_d);
+    }
+  } while (++kb < kblocks);
   wgmma_commit();
   wgmma_wait<0>();
   acc_fence(acc);
 }
 
-// R: accumulator registers per thread = the widest operator (n1_pad, n2_pad <= R)
-template <int R>
-__global__ void __launch_bounds__(128 * kMaxE + 64, 1)
+// One dispatch per chain (never per instruction) on the tile rows; the second m64 half is skipped when the tile has
+// at most 64 rows (its A rows would lie past the operand block).
+template <int N, int R>
+__device__ __forceinline__ void mma_kmajor(float (&acc)[R], int rows, uint32_t a, uint32_t a_blk, uint32_t b,
+                                           uint32_t b_blk, int kblocks) {
+  if (rows > 64) mma_chain<N, 2>(acc, a, a_blk, b, b_blk, kblocks);
+  else mma_chain<N, 1>(acc, a, a_blk, b, b_blk, kblocks);
+}
+
+// Byte offset of word y of staging row `row` (rows of Yc words, one per (kz, kt)); the chunks of 16 bytes are XORed with
+// the 128-byte line index as the destination map's swizzle mode (128 / 64 / 32 B for Yc = 32 / 16 / 8) does it, so
+// that epi-2's stores (8 rows x 4 positions per warp) spread over the banks.  swz_mask = Yc / 4 - 1.
+__device__ __forceinline__ uint32_t stg_offset(uint32_t row, uint32_t y, int Yc, uint32_t swz_mask) {
+  const uint32_t b = (row * Yc + y) * 4;
+  return b ^ (((b >> 7) & swz_mask) << 4);
+}
+
+// N1 / N2: the operator widths n1_pad / n2_pad (MMA1 / MMA2 N), chosen per launch; the accumulator holds the wider
+template <int N1, int N2>
+__global__ void __launch_bounds__(128 * max_groups(N1 > N2 ? N1 : N2) + 64, 1)
 spectral_in_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmB1,
                    const __grid_constant__ CUtensorMap tmB2, const __grid_constant__ PeerMaps pm,
                    const SpecInParams p) {
@@ -82,8 +116,7 @@ spectral_in_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constan
   uint8_t* s_ring = s_b2 + static_cast<uint32_t>(p.k2blocks) * p.n2_pad * 128;   // both operator sizes are multiples of 1024
   uint8_t* s_a2 = s_ring + p.stages * p.stage_bytes;
   uint8_t* s_stg = s_a2 + p.E * p.a2_bytes;
-  float* s_scratch = reinterpret_cast<float*>(s_stg + 2 * p.stg_bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_scratch + 4 * p.E * kRowScratchFloats);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_stg + 2 * p.stg_bytes);
   uint64_t* full = bars;                       // [kMaxStagesIn] TMA -> consumer
   uint64_t* empty = full + kMaxStagesIn;       // [kMaxStagesIn] consumer -> TMA
   uint64_t* stg_done = empty + kMaxStagesIn;   // [2] consumers -> store warp
@@ -94,7 +127,7 @@ spectral_in_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constan
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const long long n_chunks = p.rows * p.ncy;
 
-  // the K padding of A2 (columns 2T .. 16*k2steps) is never written by the epilogue: zero the buffers once
+  // the K padding of A2 (columns 2T .. 64*k2blocks) is never written by the epilogue: zero the buffers once
   {
     uint4* z0 = reinterpret_cast<uint4*>(s_a2);
     const uint32_t nz = p.E * p.a2_bytes / 16;
@@ -156,28 +189,41 @@ spectral_in_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constan
     // j mod stages (stages is a multiple of E, so every stage has one consumer and a parity wait never passes on a
     // stale phase)
     const int q = warp & 3, g = warp >> 2;
-    const int m = wg_row128(q, lane);                    // accumulator row = row of D1 and of D2
     const bool elected = q == 0 && lane == 0;
     const uint32_t barid = 1 + g;
-    float* scratch = s_scratch + warp * kRowScratchFloats;
-    // epi-1: row m = p1*T + t  ->  A2[kz*Rp + p1, 2t .. 2t+1]
-    const bool act1 = m < p.RT;
-    const int p1 = m / p.T, t1 = m - p1 * p.T;
-    const uint32_t k0 = 2 * t1;
-    const uint32_t koff = (k0 >> 6) * p.a2blk, c16 = (k0 & 63) >> 3, wi = ((k0 & 7) >> 1) * 4;
+    // Both epilogues work on the wgmma fragment: this thread holds rows m = 64 h + 16 q + lane/4 + 8 s (row slot
+    // i = 2 h + s), and registers acc[h R/2 + 4 j + 2 s + {0, 1}] are columns 8 j + 2 (lane % 4) + {0, 1}, i.e. the
+    // (re, im) pair of mode 4 j + lane % 4 (kz in D1, kt in D2): one 32-bit store each.
+    const int kc = lane & 3;
     uint8_t* a2 = s_a2 + g * p.a2_bytes;
-    // epi-2: row m = kz*Rp + p2  ->  staging[(kz*mt + kt)*Yc + tt*Rp + p2]
-    const bool act2 = m < p.RK;
-    const int kz2 = m / p.Rp, p2 = m - kz2 * p.Rp;
-    const int n1 = 2 * p.KZ, n2 = 2 * p.mt;
+    uint32_t act1 = 0, act2 = 0;                          // row slots inside the tile (m < RT for D1, m < RK for D2)
+    int p1[4], p2[4], row2[4];
+    uint32_t off1[4], c16[4], blk2[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int m = 64 * (i >> 1) + 16 * q + (lane >> 2) + 8 * (i & 1);
+      // epi-1: row m = p1*T + t  ->  A2[kz*Rp + p1, 2t .. 2t+1] (K block and word inside the 16-byte chunk, the chunk)
+      if (m < p.RT) act1 |= 1u << i;
+      p1[i] = m / p.T;
+      const uint32_t k0 = 2 * (m - p1[i] * p.T);
+      off1[i] = (k0 >> 6) * p.a2blk + ((k0 & 7) >> 1) * 4;
+      c16[i] = (k0 & 63) >> 3;
+      // epi-2: row m = kz*Rp + p2  ->  staging block of rank kz / kzl, row (kz mod kzl)*mt + kt, word tt*Rp + p2
+      if (m < p.RK) act2 |= 1u << i;
+      const int kz = m / p.Rp, jr = kz / p.kzl;
+      p2[i] = m - kz * p.Rp;
+      blk2[i] = jr * p.peer_bytes;
+      row2[i] = (kz - jr * p.kzl) * p.mt;
+    }
     const uint32_t ring_addr = smem_u32(s_ring), b1_addr = smem_u32(s_b1), b2_addr = smem_u32(s_b2);
     const uint32_t a2_addr = smem_u32(a2);
+    constexpr int R = N1 > N2 ? N1 : N2;
     int gi = 0;                                           // group of the current tile (tiles rotate over the groups)
     uint32_t cn = 0, s = 0, ph = 0;                       // chunk counter; ring stage and phase of the current tile
     mbar_wait(bfull, 0);
     float acc[R];
     for (long long chunk = blockIdx.x; chunk < n_chunks; chunk += gridDim.x, ++cn) {
-      uint32_t* stg = reinterpret_cast<uint32_t*>(s_stg + (cn & 1) * p.stg_bytes);
+      uint8_t* stg = s_stg + (cn & 1) * p.stg_bytes;
       for (int tt = 0; tt < p.tpc; ++tt) {
         const bool mine = gi == g;
         if (++gi == p.E) gi = 0;
@@ -186,49 +232,41 @@ spectral_in_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constan
         if (!mine) continue;
         // ---------------- MMA1: D1 = h tile . F1^T ----------------
         mbar_wait(&full[st], sph);
-        mma_kmajor(acc, p.n1_pad, p.RT, ring_addr + st * p.stage_bytes, p.blk1, b1_addr, p.n1_pad * 128, p.k1blocks * 4);
+        mma_kmajor<N1>(acc, p.RT, ring_addr + st * p.stage_bytes, p.blk1, b1_addr, p.n1_pad * 128, p.k1blocks);
         if (elected) mbar_arrive(&empty[st]);
         // ---------------- epi-1 ----------------
 #pragma unroll
-        for (int ch = 0; ch < R / 16; ++ch) {
-          const int c0 = ch * 16;
-          if (c0 < n1) {
-            uint32_t v[16];
-            wg_row16<2>(acc, c0, scratch, v);
-            if (act1) {
+        for (int i = 0; i < 4; ++i) {
+          if (!((act1 >> i) & 1)) continue;
+          const float* d = acc + (i >> 1) * (R / 2) + 2 * (i & 1);
 #pragma unroll
-              for (int jz = 0; jz < 8; ++jz) {
-                const int kz = (c0 >> 1) + jz;
-                if (2 * kz < n1) {
-                  const uint32_t r = static_cast<uint32_t>(kz * p.Rp + p1);
-                  *reinterpret_cast<uint32_t*>(a2 + koff + r * 128 + (((c16 ^ (r & 7)) << 4) | wi)) =
-                      pack_bf16x2(__uint_as_float(v[2 * jz]), __uint_as_float(v[2 * jz + 1]));
-                }
-              }
+          for (int j = 0; j < N1 / 8; ++j) {
+            const int kz = 4 * j + kc;
+            if (kz < p.KZ) {
+              const uint32_t r = static_cast<uint32_t>(kz * p.Rp + p1[i]);
+              *reinterpret_cast<uint32_t*>(a2 + off1[i] + r * 128 + ((c16[i] ^ (r & 7)) << 4)) =
+                  pack_bf16x2(d[4 * j], d[4 * j + 1]);
             }
           }
         }
         fence_proxy_async_smem();
         asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
         // ---------------- MMA2: D2 = A2 . F2^T ----------------
-        mma_kmajor(acc, p.n2_pad, p.RK, a2_addr, p.a2blk, b2_addr, p.n2_pad * 128, p.k2steps);
+        mma_kmajor<N2>(acc, p.RK, a2_addr, p.a2blk, b2_addr, p.n2_pad * 128, p.k2blocks);
         // ---------------- epi-2 ----------------
         mbar_wait_warp(&stg_free[cn & 1], ((cn >> 1) & 1) ^ 1);
 #pragma unroll
-        for (int ch = 0; ch < R / 16; ++ch) {
-          const int c0 = ch * 16;
-          if (c0 < n2) {
-            uint32_t v[16];
-            wg_row16<2>(acc, c0, scratch, v);
-            if (act2) {
+        for (int i = 0; i < 4; ++i) {
+          if (!((act2 >> i) & 1)) continue;
+          const float* d = acc + (i >> 1) * (R / 2) + 2 * (i & 1);
+          uint8_t* blk = stg + blk2[i];
+          const uint32_t y = static_cast<uint32_t>(tt * p.Rp + p2[i]);
 #pragma unroll
-              for (int jt = 0; jt < 8; ++jt) {
-                const int kt = (c0 >> 1) + jt;
-                if (kt < p.mt)
-                  stg[(kz2 * p.mt + kt) * p.Yc + tt * p.Rp + p2] =
-                      pack_bf16x2(__uint_as_float(v[2 * jt]), __uint_as_float(v[2 * jt + 1]));
-              }
-            }
+          for (int j = 0; j < N2 / 8; ++j) {
+            const int kt = 4 * j + kc;
+            if (kt < p.mt)
+              *reinterpret_cast<uint32_t*>(blk + stg_offset(row2[i] + kt, y, p.Yc, p.swz)) =
+                  pack_bf16x2(d[4 * j], d[4 * j + 1]);
           }
         }
         fence_proxy_async_smem();
@@ -238,6 +276,28 @@ spectral_in_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constan
     }
   }
 }
+
+template <int N1, int N2>
+cudaError_t launch_spectral_in(int grid, int threads, uint32_t smem_bytes, cudaStream_t stream, const CUtensorMap& tmH,
+                               const CUtensorMap& tmB1, const CUtensorMap& tmB2, const PeerMaps& pm, const SpecInParams& p) {
+  static bool attr = false;
+  if (!attr) {
+    const cudaError_t e = cudaFuncSetAttribute(spectral_in_kernel<N1, N2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    attr = true;
+  }
+  spectral_in_kernel<N1, N2><<<grid, threads, smem_bytes, stream>>>(tmH, tmB1, tmB2, pm, p);
+  return cudaGetLastError();
+}
+
+// one instantiation per (n1_pad, MMA2 width class): n1_pad = 16 .. 128, N2 = 16, 32, 48, 64, 80, 128
+using SpecInLaunch = decltype(&launch_spectral_in<16, 16>);
+#define DFNO_ROW(N1)                                                                                            \
+  {&launch_spectral_in<N1, 16>, &launch_spectral_in<N1, 32>, &launch_spectral_in<N1, 48>,                      \
+   &launch_spectral_in<N1, 64>, &launch_spectral_in<N1, 80>, &launch_spectral_in<N1, 128>}
+constexpr SpecInLaunch kLaunch[8][6] = {DFNO_ROW(16), DFNO_ROW(32), DFNO_ROW(48), DFNO_ROW(64),
+                                        DFNO_ROW(80), DFNO_ROW(96), DFNO_ROW(112), DFNO_ROW(128)};
+#undef DFNO_ROW
 
 inline uint32_t align_up_u32(uint32_t v, uint32_t a) { return (v + a - 1) / a * a; }
 
@@ -258,12 +318,12 @@ const char* plan_spectral_in(SpecInParams& p, int n1_pad, int k1_pad, int n2_pad
   if (p.rows > (1ll << 30)) return "spectral_in: tensor too large";
   p.X = X; p.T = T; p.KZ = KZ; p.mt = mt; p.P = P; p.kzl = KZ / P;
   p.k1blocks = k1_pad / 64; p.n1_pad = n1_pad;
-  p.k2steps = (2 * T + 15) / 16; p.k2blocks = (p.k2steps + 3) / 4; p.n2_pad = n2_pad;
+  p.k2blocks = (2 * T + 63) / 64; p.n2_pad = n2_pad;
   if (p.k2blocks * 64 > k2_pad) return "spectral_in: operator 2 is narrower than its reduction";
   const uint32_t ops_bytes = static_cast<uint32_t>(p.k1blocks) * n1_pad * 128 + static_cast<uint32_t>(p.k2blocks) * n2_pad * 128;
   if ((static_cast<uint32_t>(p.k1blocks) * n1_pad * 128) % 1024 || ops_bytes % 1024) return "spectral_in: operator rows must be a multiple of 8";
-  const uint32_t budget = 227 * 1024 - 1024 /*align*/ - 512 /*barriers*/;
   const int rmax = (128 / T) < (128 / KZ) ? (128 / T) : (128 / KZ);
+  const int max_e = max_groups(n1_pad > mma2_width(n2_pad) ? n1_pad : mma2_width(n2_pad));
   bool ok = false;
   for (int min_st = 3; min_st >= 2 && !ok; --min_st)       // prefer a deep TMA ring and two epilogue groups
   for (int Rp = 4; Rp >= 1 && !ok; Rp >>= 1) {
@@ -272,20 +332,31 @@ const char* plan_spectral_in(SpecInParams& p, int n1_pad, int k1_pad, int n2_pad
     while (yc > 4 && yc / 2 >= Yl) yc >>= 1;                   // the smallest of {4, 8, 16, 32} covering Yl, 32 beyond
     for (; yc >= 4 && !ok; yc >>= 1) {
       if (yc % Rp) continue;
-      const uint32_t peer_bytes = static_cast<uint32_t>(p.kzl) * mt * yc * 4;
-      if (peer_bytes % 128) continue;
-      const uint32_t stg_bytes = align_up_u32(peer_bytes * P, 1024);
+      const uint32_t peer_dense = static_cast<uint32_t>(p.kzl) * mt * yc * 4;
+      if (peer_dense % 128) continue;
+      // swizzled staging (yc >= 8) starts every rank's block on a 1024-byte boundary, where the swizzle pattern starts
+      const uint32_t peer_swz = yc >= 8 ? align_up_u32(peer_dense, 1024) : peer_dense;
       const uint32_t blk1 = align_up_u32(static_cast<uint32_t>(Rp) * T * 128, 1024);
       const uint32_t a2blk = align_up_u32(static_cast<uint32_t>(Rp) * KZ * 128, 1024);
-      for (int E = kMaxE; E >= 1 && !ok; --E) {
-        for (int st = 5; st >= 2; --st) {
+      for (int E = max_e; E >= 1 && !ok; --E) {
+        for (int st = kMaxStagesIn; st >= 2; --st) {
           if (st % E) continue;                                  // every ring stage belongs to one warpgroup
-          const uint32_t need = ops_bytes + st * p.k1blocks * blk1 + E * p.k2blocks * a2blk + 2 * stg_bytes +
-                                4u * E * kRowScratchFloats * 4;
-          if (need <= budget && st >= min_st && (E >= 2 || min_st == 2)) {
+          const uint32_t ring_end = ops_bytes + st * p.k1blocks * blk1, a2_end = ring_end + E * p.k2blocks * a2blk;
+          // a wgmma reads whole m64 halves, i.e. up to 64 (128) rows from the last K block of the last ring stage
+          // and A2 buffer, past the rows a tile fills: those reads have to stay inside the allocation
+          const uint32_t reach = std::max(ring_end - blk1 + (Rp * T > 64 ? 128u : 64u) * 128,
+                                          a2_end - a2blk + (Rp * KZ > 64 ? 128u : 64u) * 128);
+          auto smem_for = [&](uint32_t stg) { return std::max(a2_end + 2 * stg + 512 /*barriers*/, reach) + 1024 /*align*/; };
+          // dense (bank-conflicted) staging only where the padding of the swizzled one does not fit
+          const bool swizzled = smem_for(align_up_u32(peer_swz * P, 1024)) <= 227u * 1024;
+          const uint32_t peer_bytes = swizzled ? peer_swz : peer_dense;
+          const uint32_t stg_bytes = align_up_u32(peer_bytes * P, 1024);
+          if (smem_for(stg_bytes) <= 227u * 1024 && st >= min_st && (E >= 2 || min_st == 2)) {
+            p.smem_bytes = smem_for(stg_bytes);
             p.Rp = Rp; p.Yc = yc; p.E = E; p.stages = st; p.blk1 = blk1; p.a2blk = a2blk;
             p.stage_bytes = p.k1blocks * blk1; p.a2_bytes = p.k2blocks * a2blk; p.stg_bytes = stg_bytes;
             p.peer_bytes = peer_bytes;
+            p.swz = swizzled ? static_cast<uint32_t>(yc / 4 - 1) : 0u;
             ok = true;
             break;
           }
@@ -319,7 +390,6 @@ const char* spectral_in(const void* h, const void* op1, int n1_pad, int k1_pad, 
                         int Yl, int T, int Z, int KZ, int mt, int num_sms, cudaStream_t stream) {
   SpecInParams p;
   if (const char* err = plan_spectral_in(p, n1_pad, k1_pad, n2_pad, k2_pad, P, dst_off, dstr, BC, X, Yl, T, Z, KZ, mt)) return err;
-  const uint32_t ops_bytes = static_cast<uint32_t>(p.k1blocks) * n1_pad * 128 + static_cast<uint32_t>(p.k2blocks) * n2_pad * 128;
   CUtensorMap tmH, tmB1, tmB2;
   PeerMaps pm;
   if (make_map_3d(&tmH, h, Z, static_cast<uint64_t>(Yl) * T, p.rows, Z, static_cast<uint64_t>(Yl) * T * Z, 64, p.RT, 1))
@@ -334,26 +404,15 @@ const char* spectral_in(const void* h, const void* op1, int n1_pad, int k1_pad, 
                              static_cast<uint64_t>(dstr[3])};
     const uint32_t box[5] = {static_cast<uint32_t>(p.Yc) * 2, 1, static_cast<uint32_t>(mt), static_cast<uint32_t>(p.kzl), 1};
     const void* base = reinterpret_cast<const void*>(static_cast<uintptr_t>(dst_ptrs[jj]) + static_cast<uintptr_t>(dst_off) * 2);
-    if (make_map_nd_plain(&pm.m[j], base, 5, dims, str, box)) return "tensor map (destination) failed";
+    const CUtensorMapSwizzle swz = p.swz == 7 ? CU_TENSOR_MAP_SWIZZLE_128B : p.swz == 3 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                 : p.swz == 1 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE;
+    if (make_map_nd(&pm.m[j], base, 5, dims, str, box, swz)) return "tensor map (destination) failed";
   }
-  const uint32_t smem_bytes = ops_bytes + p.stages * p.stage_bytes + p.E * p.a2_bytes + 2 * p.stg_bytes +
-                              4u * p.E * kRowScratchFloats * 4 + 512 + 1024;
   const long long chunks = p.rows * p.ncy;
   const int grid = static_cast<int>(chunks < num_sms ? chunks : num_sms);
   const int threads = 128 * p.E + 64;
-  const uint32_t dyn = smem_bytes;
-  const bool narrow = n1_pad <= 64 && n2_pad <= 64;
-  static bool attr[2] = {false, false};
-  const void* fn = narrow ? reinterpret_cast<const void*>(spectral_in_kernel<64>)
-                          : reinterpret_cast<const void*>(spectral_in_kernel<128>);
-  if (!attr[narrow]) {
-    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-      return "cudaFuncSetAttribute failed";
-    attr[narrow] = true;
-  }
-  if (narrow) spectral_in_kernel<64><<<grid, threads, dyn, stream>>>(tmH, tmB1, tmB2, pm, p);
-  else spectral_in_kernel<128><<<grid, threads, dyn, stream>>>(tmH, tmB1, tmB2, pm, p);
-  cudaError_t e = cudaGetLastError();
+  const int i1 = n1_pad / 16 - 1, i2 = mma2_width(n2_pad) / 16 - 1 - (n2_pad > 80 ? 2 : 0);
+  const cudaError_t e = kLaunch[i1][i2](grid, threads, p.smem_bytes, stream, tmH, tmB1, tmB2, pm, p);
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 

@@ -55,11 +55,11 @@ inline int make_map_3d(CUtensorMap* m, const void* base, uint64_t d0, uint64_t d
   return r == CUDA_SUCCESS ? 0 : static_cast<int>(r);
 }
 
-// rank-N (<= 5) bf16 tensor map WITHOUT swizzle (dense shared-memory box, innermost dimension first): used for
-// stores whose staging buffer is written with plain word stores.  `strides` (elements) belong to dims 1..rank-1
-// and must be multiples of 8; box[0] * 2 bytes must be a multiple of 16.  Stores are clipped at the extents.
-inline int make_map_nd_plain(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
-                             const uint32_t* box) {
+// rank-N (<= 5) bf16 tensor map, innermost dimension first: used for stores whose staging buffer is written with word
+// stores.  `strides` (elements) belong to dims 1..rank-1 and must be multiples of 8; box[0] * 2 bytes must be a
+// multiple of 16 and, with a swizzle, at most its span (32 / 64 / 128 B).  Stores are clipped at the extents.
+inline int make_map_nd(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
+                       const uint32_t* box, CUtensorMapSwizzle swizzle) {
   PFN_encodeTiled enc = get_encode_fn();
   if (!enc || rank < 1 || rank > 5) return -1;
   cuuint64_t d[5], st[4];
@@ -67,7 +67,7 @@ inline int make_map_nd_plain(CUtensorMap* m, const void* base, int rank, const u
   for (int i = 0; i < rank; ++i) { d[i] = dims[i]; b[i] = box[i]; estr[i] = 1; }
   for (int i = 0; i + 1 < rank; ++i) st[i] = strides[i] * 2;
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, static_cast<cuuint32_t>(rank), const_cast<void*>(base), d, st, b,
-                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : static_cast<int>(r);
 }
