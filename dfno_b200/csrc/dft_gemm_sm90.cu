@@ -6,9 +6,10 @@
 // K = the transformed axis, N = the retained modes -- a tiny operator B applied to a huge streamed A.  B stays
 // resident in shared memory; A tiles stream through one TMA/mbarrier ring per consumer warpgroup; a consumer
 // warpgroup issues the wgmma chain of a whole tile (128 rows for N <= 128, 64 rows for N <= 256) and runs its
-// epilogue: a row-major tile (optionally adding a bf16 tensor) or a scattered, transposed layout through a
-// mixed-radix address table, possibly into a peer GPU's symmetric buffer (the fused pencil transposes).
-// Memory bound by construction (AI ~ N flop/byte): the tensor core only has to stay off the critical path.
+// epilogue on the accumulator fragments: a row-major tile (optionally adding a bf16 tensor) or a scattered, transposed
+// layout through a mixed-radix address table, possibly into a peer GPU's symmetric buffer (the fused pencil
+// transposes).  Memory bound by construction (AI ~ N flop/byte): the tensor core only has to stay off the critical
+// path.  The kernel is instantiated per padded operator width, so that each chain's wgmmas issue back to back.
 #include "sm90_ptx.cuh"
 #include "dft_gemm.h"
 #include "tma_host.h"
@@ -16,17 +17,22 @@
 namespace dfno {
 
 static constexpr int kBlockK = 64;                 // bf16 elements per 128-byte swizzle row
-static constexpr int kMaxGroups = 2;               // consumer warpgroups (128 accumulator registers each)
-static constexpr int kMaxThreads = 128 * kMaxGroups + 32;
 static constexpr int kMaxStagesPerGroup = 4;       // A-tile ring depth of one consumer: bytes in flight per SM must
                                                    // cover HBM latency x bandwidth share (~40 KB)
+static constexpr int kMaxStages = 16;              // ring stages of all consumer warpgroups (mbarrier pairs)
+
+// Tile geometry of the instantiation for padded width n_pad: 128-row tiles (two m64 halves) up to 128 columns, 64-row
+// tiles beyond; the accumulator holds kHalves * n_pad / 2 registers.  Consumer warpgroups: four while the
+// accumulator takes at most 64 registers, two beyond (the register file of one CTA per SM).
+constexpr int dft_halves(int n_pad) { return n_pad <= 128 ? 2 : 1; }
+constexpr int dft_acc_regs(int n_pad) { return dft_halves(n_pad) * n_pad / 2; }
+constexpr int dft_max_groups(int n_pad) { return dft_acc_regs(n_pad) <= 64 ? 3 : 2; }
 
 struct SmemLayout {
   uint32_t b_bytes;       // kblocks * n_pad * 128
   uint32_t a_tile_bytes;  // bytes of one ring stage = kbs * MT * 128
   uint32_t kbs;           // 64-wide K blocks per ring stage (= kblocks unless the whole-K tile is too large)
   uint32_t spg;           // ring stages per consumer warpgroup
-  uint32_t scratch_off;   // byte offset of the per-warp row-view scratch
   uint32_t stage_off;     // byte offset of the epilogue staging area
   uint32_t stage_pitch;   // bytes per staged row (+16 B pad); 0 = direct stores
 };
@@ -60,23 +66,28 @@ __device__ __forceinline__ long long row_offset(const EpiParams& e, uint32_t r, 
   return off;
 }
 
-// kHalves = 2: 128-row tiles (n_pad <= 128); 1: 64-row tiles (n_pad <= 256)
-template <int kHalves>
-__global__ void __launch_bounds__(kMaxThreads, 1)
+// Accumulator fragment (sm90_ptx.cuh, wgmma D layout): thread (warp q of its warpgroup, lane l) holds, in m64 half h
+// and for i = 0, 1, the tile row 64h + 16q + l/4 + 8i; register h * kN/2 + 4j + 2i + {0, 1} is column 8j + 2(l%4) + {0, 1}
+// of that row, i.e. the (re, im) pair 4j + l%4.
+template <int kN>
+__global__ void __launch_bounds__(128 * dft_max_groups(kN) + 32, 1)
 dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const GemmParams p, const SmemLayout L) {
+  constexpr int kHalves = dft_halves(kN);
   constexpr int kTileM = 64 * kHalves;
-  constexpr int kWarpRows = 16 * kHalves;            // rows of a tile held by one warp
+  constexpr int kAcc = dft_acc_regs(kN);
+  constexpr int kHalfRegs = kN / 2;                  // registers of one m64 half
+  constexpr int kRows = 2 * kHalves;                 // tile rows held by one thread
   extern __shared__ __align__(1024) uint8_t smem[];
   const int E = (static_cast<int>(blockDim.x) - 32) >> 7;     // consumer warpgroups
   const int spg = static_cast<int>(L.spg);
   uint8_t* smem_b = smem;
   uint8_t* smem_a = smem + L.b_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_a + E * spg * L.a_tile_bytes);
-  uint64_t* full = bars;                      // [E * spg]   TMA -> consumer
-  uint64_t* empty = bars + 8;                 // [E * spg]   consumer -> TMA
-  uint64_t* bfull = bars + 16;                // [1]   B resident
-  long long* s_coloff = reinterpret_cast<long long*>(bars + 24);        // [128] pair -> element offset
+  uint64_t* full = bars;                              // [E * spg]   TMA -> consumer
+  uint64_t* empty = bars + kMaxStages;                // [E * spg]   consumer -> TMA
+  uint64_t* bfull = bars + 2 * kMaxStages;            // [1]   B resident
+  long long* s_coloff = reinterpret_cast<long long*>(bars + 2 * kMaxStages + 8);   // [128] pair -> element offset
   float* s_vec = reinterpret_cast<float*>(s_coloff + 128);              // [512] EPI_HEAD vectors
   uint8_t* s_colpeer = reinterpret_cast<uint8_t*>(s_vec + 512);         // [128] pair -> peer
 
@@ -100,28 +111,24 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
   if (warp == 4 * E) {
     // ===================== TMA producer (one lane) =====================
-    // tile n of this CTA goes to warpgroup n % E, through that warpgroup's own ring (each ring is filled and
-    // drained in order, so a parity wait can never pass on a phase two fills ahead)
+    // the n-th tile of this CTA goes to warpgroup n % E, through that warpgroup's own ring as its (n / E)-th tile
+    // (each ring is filled and drained in order, so a parity wait can never pass on a phase two fills ahead)
     if (lane == 0) {
       mbar_arrive_expect_tx(bfull, L.b_bytes);
       for (int kb = 0; kb < kblocks; ++kb)
         tma_load_2d(smem_b + kb * p.n_pad * 128, &tmB, bfull, kb * kBlockK, 0);
-      uint32_t slot = 0, ph = 0, slot_o = 0, ph_o = 0;         // ring position of this / the other warpgroup
-      int g = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        for (int kb0 = 0; kb0 < kblocks; kb0 += kbs) {          // one ring stage per K chunk (usually the whole K)
-          const uint32_t s = g * spg + slot;
+      const uint32_t chunks = static_cast<uint32_t>(kblocks / kbs);   // ring stages per tile
+      uint32_t n = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
+        const uint32_t g = n % static_cast<uint32_t>(E);
+        uint32_t fill = (n / static_cast<uint32_t>(E)) * chunks;      // this warpgroup's ring fills so far
+        for (int kb0 = 0; kb0 < kblocks; kb0 += kbs, ++fill) {       // one ring stage per K chunk (usually the whole K)
+          const uint32_t s = g * spg + fill % spg, ph = (fill / spg) & 1;
           mbar_wait(&empty[s], ph ^ 1);
           mbar_arrive_expect_tx(&full[s], L.a_tile_bytes);
           uint8_t* dst = smem_a + s * L.a_tile_bytes;
           for (int kb = 0; kb < kbs; ++kb)
             tma_load_2d(dst + kb * (kTileM * 128), &tmA, &full[s], (kb0 + kb) * kBlockK, tile * kTileM);
-          if (++slot == static_cast<uint32_t>(spg)) { slot = 0; ph ^= 1; }
-        }
-        if (E == 2) {
-          g ^= 1;
-          const uint32_t ts = slot, tp = ph;
-          slot = slot_o; ph = ph_o; slot_o = ts; ph_o = tp;
         }
       }
     }
@@ -131,9 +138,6 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   // ===================== consumer warpgroups: wgmma chain + epilogue =====================
   const int g = warp >> 2;                                     // warpgroup
   const int q = warp & 3;                                      // warp inside the warpgroup
-  const int r_in_tile = kHalves == 2 ? wg_row128(q, lane) : 16 * q + lane;
-  const bool lane_has_row = kHalves == 2 || lane < 16;
-  float* scratch = reinterpret_cast<float*>(smem + L.scratch_off) + warp * kRowScratchFloats;
   const int npairs = p.N >> 1;
   {
     // per-CTA lookup tables (all consumer threads; named barrier 1)
@@ -154,69 +158,60 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     asm volatile("bar.sync 1, %0;" ::"r"(nthr) : "memory");
   }
   mbar_wait(bfull, 0);
-  const int ksteps = (p.K + 15) / 16;                          // K=16 per instruction; zero tail needs no MMA
   const uint32_t b_addr = smem_u32(smem_b);
-  float acc[kAccRegs];
+  const int quad = lane & 3;
+  float acc[kAcc];
   uint32_t slot = 0, ph = 0;
   for (int tile = blockIdx.x + g * gridDim.x; tile < num_tiles; tile += E * gridDim.x) {
     for (int kb0 = 0; kb0 < kblocks; kb0 += kbs) {
       const uint32_t s = g * spg + slot;
-      mbar_wait(&full[s], ph);
-      const uint32_t a_addr = smem_u32(smem_a + s * L.a_tile_bytes);
-      const int ks_end = min(ksteps, (kb0 + kbs) * 4);
-      wgmma_fence();
-      for (int ks = kb0 * 4; ks < ks_end; ++ks) {
-        const uint32_t kb = ks >> 2, kk = ks & 3;
-        const uint64_t da = gdesc_k128(a_addr + (kb - kb0) * (kTileM * 128) + kk * 32);
-        const uint64_t db = gdesc_k128(b_addr + kb * p.n_pad * 128 + kk * 32);
-        if (kHalves == 2) wg_mma128<false, 0, 0>(acc, p.n_pad, da, 8192, db, ks > 0 ? 1u : 0u);
-        else wg_mma64<false, 0, 0, 0>(acc, p.n_pad, da, db, ks > 0 ? 1u : 0u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      acc_fence(acc);
+      mbar_wait_warp(&full[s], ph);
+      // whole K blocks: the zero K tail inside the last block (TMA zero-fills A past K) costs no memory traffic
+      mma_chain<kN, kHalves>(acc, smem_u32(smem_a + s * L.a_tile_bytes), kTileM * 128, b_addr + kb0 * kN * 128,
+                             kN * 128, kbs, kb0 > 0);
       if ((threadIdx.x & 127) == 0) mbar_arrive(&empty[s]);       // the ring stage may be refilled
       if (++slot == static_cast<uint32_t>(spg)) { slot = 0; ph ^= 1; }
     }
-    const long long row = static_cast<long long>(tile) * kTileM + r_in_tile;
-    const bool row_ok = lane_has_row && row < p.M;
+    const long long tile0 = static_cast<long long>(tile) * kTileM;
+    // tile row of this thread's fragment row r = 2h + i, and its row in the warp's staging slab
+    auto frag_row = [&](int r) { return 64 * (r >> 1) + 16 * q + (lane >> 2) + 8 * (r & 1); };
 
     if (p.epi.mode == EPI_ROWMAJOR && L.stage_pitch != 0) {
-      // ---- coalesced row-major store: accumulator -> staging rows in smem (a private slab per warp holding its
-      // kWarpRows rows, lane r = row r of the warp) -> groups of lanes write whole rows contiguously
+      // ---- coalesced row-major store: fragments -> staging rows in smem (a private slab per warp holding its
+      // 16 * kHalves rows: slab row 16h + r' = tile row 64h + 16q + r') -> groups of lanes write whole rows contiguously
       uint8_t* slab = smem + L.stage_off + (warp * 32) * L.stage_pitch;
-      uint8_t* myrow = slab + lane * L.stage_pitch;
       const bool st16 = !p.epi.out_fp32;                       // bf16 output: stage packed bf16
+      const uint32_t slab_addr = smem_u32(slab);
 #pragma unroll
-      for (int ch = 0; ch < 8 * (3 - kHalves); ++ch) {
-        const int c0 = ch * 16;
-        if (c0 < p.N) {
-          uint32_t v[16];
-          wg_row16<kHalves>(acc, c0, scratch, v);
+      for (int h = 0; h < kHalves; ++h) {
+#pragma unroll
+        for (int c = 0; c < kN / 16; ++c) {
+          if (16 * c >= p.N) continue;
+          const float* a = acc + h * kHalfRegs + 8 * c;
           if (st16) {
-            uint4 u0, u1;
-            u0.x = pack_bf16x2(__uint_as_float(v[0]), __uint_as_float(v[1]));
-            u0.y = pack_bf16x2(__uint_as_float(v[2]), __uint_as_float(v[3]));
-            u0.z = pack_bf16x2(__uint_as_float(v[4]), __uint_as_float(v[5]));
-            u0.w = pack_bf16x2(__uint_as_float(v[6]), __uint_as_float(v[7]));
-            u1.x = pack_bf16x2(__uint_as_float(v[8]), __uint_as_float(v[9]));
-            u1.y = pack_bf16x2(__uint_as_float(v[10]), __uint_as_float(v[11]));
-            u1.z = pack_bf16x2(__uint_as_float(v[12]), __uint_as_float(v[13]));
-            u1.w = pack_bf16x2(__uint_as_float(v[14]), __uint_as_float(v[15]));
-            reinterpret_cast<uint4*>(myrow + c0 * 2)[0] = u0;
-            reinterpret_cast<uint4*>(myrow + c0 * 2)[1] = u1;
+            // four 8 x 8 matrices: rows 0-7 / 8-15 x columns 16c .. +7 / 16c + 8 .. +15
+            const uint32_t r[4] = {pack_bf16x2(a[0], a[1]), pack_bf16x2(a[2], a[3]), pack_bf16x2(a[4], a[5]),
+                                   pack_bf16x2(a[6], a[7])};
+            const int mi = lane >> 3;
+            const uint32_t row = 16 * h + (lane & 7) + 8 * (mi & 1);
+            stmatrix_x4(slab_addr + row * L.stage_pitch + (16 * c + 8 * (mi >> 1)) * 2, r);
           } else {
 #pragma unroll
-            for (int i = 0; i < 4; ++i)
-              reinterpret_cast<uint4*>(myrow + c0 * 4)[i] = make_uint4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+            for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                const int row = 16 * h + (lane >> 2) + 8 * i;
+                *reinterpret_cast<float2*>(slab + row * L.stage_pitch + (16 * c + 8 * jj + 2 * quad) * 4) =
+                    make_float2(a[4 * jj + 2 * i], a[4 * jj + 2 * i + 1]);
+              }
           }
         }
       }
       __syncwarp();
+      constexpr int kWarpRows = 16 * kHalves;                 // rows of a tile held by one warp
       const int vec_per_row = p.N >> 3;                       // 8 outputs per lane
       const int rows_per_it = 32 / vec_per_row;               // N = 128 -> 16 lanes per row, 2 rows / instr
       const int lr = lane / vec_per_row, lc = lane % vec_per_row;
-      const long long tile0 = static_cast<long long>(tile) * kTileM;
       for (int rb = lr; rb < kWarpRows; rb += 4 * rows_per_it) {
         uint4 addv[4];
         bool okv[4];
@@ -224,7 +219,7 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 #pragma unroll
         for (int u = 0; u < 4; ++u) {                          // issue all global loads first
           const int rr = rb + u * rows_per_it;
-          growv[u] = tile0 + (kHalves == 2 ? wg_row128(q, rr) : 16 * q + rr);
+          growv[u] = tile0 + 64 * (rr >> 4) + 16 * q + (rr & 15);
           okv[u] = rr < kWarpRows && growv[u] < p.M;
           addv[u] = make_uint4(0, 0, 0, 0);
           if (okv[u] && p.epi.add_src != nullptr)
@@ -263,90 +258,99 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       }
       __syncwarp();                                            // slab reusable by this warp's next tile
     } else if (p.epi.mode == EPI_ROWMAJOR) {
+      // ---- direct row-major store: each (re, im)-adjacent register pair is two consecutive columns of one row
 #pragma unroll
-      for (int ch = 0; ch < 8 * (3 - kHalves); ++ch) {
-        const int c0 = ch * 16;
-        if (c0 >= p.N) continue;
-        uint32_t v[16];
-        wg_row16<kHalves>(acc, c0, scratch, v);
-        if (!row_ok) continue;
-        float f[16];
+      for (int r = 0; r < kRows; ++r) {
+        const long long row = tile0 + frag_row(r);
+        if (row >= p.M) continue;
+        const float* a = acc + (r >> 1) * kHalfRegs + 2 * (r & 1);
 #pragma unroll
-        for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(v[i]);
-        const int ncol = min(16, p.N - c0);
-        const bool vec = p.epi.vec_ok && ncol == 16;
-        if (p.epi.add_src != nullptr) {
-          const __nv_bfloat16* ap = reinterpret_cast<const __nv_bfloat16*>(p.epi.add_src) + row * p.epi.ld_add + c0;
-          for (int i = 0; i < ncol; ++i) f[i] += __bfloat162float(ap[i]);
-        }
-        if (p.epi.out_fp32) {
-          float* o = reinterpret_cast<float*>(p.epi.peers[0]) + row * p.epi.ldc + c0;
-          if (vec) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              reinterpret_cast<float4*>(o)[i] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
-          } else {
-            for (int i = 0; i < ncol; ++i) o[i] = f[i];
+        for (int j = 0; j < kN / 8; ++j) {
+          const int col = 8 * j + 2 * quad;
+          if (col >= p.N) continue;
+          float f0 = a[4 * j], f1 = a[4 * j + 1];
+          const bool two = col + 1 < p.N;
+          const bool vec = p.epi.vec_ok && two;               // 8 / 4-byte aligned: ldc, ld_add and bases are 16 B
+          if (p.epi.add_src != nullptr) {
+            const __nv_bfloat16* ap = reinterpret_cast<const __nv_bfloat16*>(p.epi.add_src) + row * p.epi.ld_add + col;
+            if (vec) {
+              const float2 t = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(ap));
+              f0 += t.x; f1 += t.y;
+            } else {
+              f0 += __bfloat162float(ap[0]);
+              if (two) f1 += __bfloat162float(ap[1]);
+            }
           }
-        } else {
-          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.epi.peers[0]) + row * p.epi.ldc + c0;
-          if (vec) {
-            uint4 u0, u1;
-            u0.x = pack_bf16x2(f[0], f[1]);   u0.y = pack_bf16x2(f[2], f[3]);
-            u0.z = pack_bf16x2(f[4], f[5]);   u0.w = pack_bf16x2(f[6], f[7]);
-            u1.x = pack_bf16x2(f[8], f[9]);   u1.y = pack_bf16x2(f[10], f[11]);
-            u1.z = pack_bf16x2(f[12], f[13]); u1.w = pack_bf16x2(f[14], f[15]);
-            reinterpret_cast<uint4*>(o)[0] = u0;
-            reinterpret_cast<uint4*>(o)[1] = u1;
+          if (p.epi.out_fp32) {
+            float* o = reinterpret_cast<float*>(p.epi.peers[0]) + row * p.epi.ldc + col;
+            if (vec) {
+              *reinterpret_cast<float2*>(o) = make_float2(f0, f1);
+            } else {
+              o[0] = f0;
+              if (two) o[1] = f1;
+            }
           } else {
-            for (int i = 0; i < ncol; ++i) o[i] = __float2bfloat16(f[i]);
+            __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.epi.peers[0]) + row * p.epi.ldc + col;
+            if (vec) {
+              *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(f0, f1);
+            } else {
+              o[0] = __float2bfloat16(f0);
+              if (two) o[1] = __float2bfloat16(f1);
+            }
           }
         }
       }
     } else if (p.epi.mode == EPI_PAIR_SCATTER) {
-      // ---- pair scatter: (re, im) pairs to a mixed-radix address, possibly on a peer GPU
-      int rpeer;
-      const long long roff = row_offset(p.epi, static_cast<uint32_t>(row_ok ? row : 0), rpeer);
-      __nv_bfloat16* const rbase = reinterpret_cast<__nv_bfloat16*>(p.epi.peers[rpeer]) + roff;
+      // ---- pair scatter: each register pair is one (re, im) pair, stored as one 32-bit word at a mixed-radix
+      // address, possibly on a peer GPU.  A warp's store covers 8 consecutive rows x 4 pairs.
+      // Byte address = row part + column part; the peer buffer's base goes with the digit that selects it.
+      const bool by_col = p.epi.peer_sel == PEER_BY_COL;
+      uint64_t rbase[kRows];
+      bool rok[kRows];
 #pragma unroll
-      for (int ch = 0; ch < 8 * (3 - kHalves); ++ch) {
-        const int c0 = ch * 16;
-        if (c0 >= p.N) continue;
-        uint32_t v[16];
-        wg_row16<kHalves>(acc, c0, scratch, v);
-        if (!row_ok) continue;
+      for (int r = 0; r < kRows; ++r) {
+        const long long row = tile0 + frag_row(r);
+        int rpeer;
+        rok[r] = row < p.M;
+        const long long roff = row_offset(p.epi, static_cast<uint32_t>(rok[r] ? row : 0), rpeer);
+        rbase[r] = (by_col ? 0ull : reinterpret_cast<uint64_t>(p.epi.peers[rpeer])) + 2ull * roff;
+      }
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int j = (c0 >> 1) + i;
-          if (j < npairs) {
-            __nv_bfloat16* base = rbase;
-            if (p.epi.peer_sel == PEER_BY_COL)
-              base = reinterpret_cast<__nv_bfloat16*>(p.epi.peers[s_colpeer[j]]) + roff;
-            *reinterpret_cast<uint32_t*>(base + s_coloff[j]) =
-                pack_bf16x2(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]));
-          }
+      for (int j = 0; j < kN / 8; ++j) {
+        const int jp = 4 * j + quad;
+        if (jp >= npairs) continue;
+        const uint64_t cadd = (by_col ? reinterpret_cast<uint64_t>(p.epi.peers[s_colpeer[jp]]) : 0ull) +
+                              2ull * s_coloff[jp];
+#pragma unroll
+        for (int r = 0; r < kRows; ++r) {
+          if (!rok[r]) continue;
+          const float* a = acc + (r >> 1) * kHalfRegs + 4 * j + 2 * (r & 1);
+          *reinterpret_cast<uint32_t*>(rbase[r] + cadd) = pack_bf16x2(a[0], a[1]);
         }
       }
     } else {
-      // ---- projection head: out = b4 + sum_j W4[j] * gelu(acc[j] + b3[j])
-      float part = s_vec[511];
+      // ---- projection head: out = b4 + sum_j W4[j] * gelu(acc[j] + b3[j]); the four lanes of a quad hold the
+      // columns of the same rows and are reduced with shuffles
 #pragma unroll
-      for (int ch = 0; ch < 8 * (3 - kHalves); ++ch) {
-        const int c0 = ch * 16;
-        if (c0 >= p.N) continue;
-        uint32_t v[16];
-        wg_row16<kHalves>(acc, c0, scratch, v);
+      for (int r = 0; r < kRows; ++r) {
+        const float* a = acc + (r >> 1) * kHalfRegs + 2 * (r & 1);
+        float part = 0.f;
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          if (c0 + i < p.N) {
-            const float pre = __uint_as_float(v[i]) + s_vec[c0 + i];
-            part = fmaf(s_vec[256 + c0 + i], gelu_erf(pre), part);
+        for (int j = 0; j < kN / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * j + 2 * quad + e;
+            if (col < p.N) part = fmaf(s_vec[256 + col], gelu_erf(a[4 * j + e] + s_vec[col]), part);
           }
         }
-      }
-      if (row_ok) {
-        int unused;
-        reinterpret_cast<float*>(p.epi.peers[0])[row_offset(p.epi, static_cast<uint32_t>(row), unused)] = part;
+        part += __shfl_xor_sync(0xffffffffu, part, 1);
+        part += __shfl_xor_sync(0xffffffffu, part, 2);
+        const long long row = tile0 + frag_row(r);
+        if (quad == 0 && row < p.M) {
+          int unused;
+          reinterpret_cast<float*>(p.epi.peers[0])[row_offset(p.epi, static_cast<uint32_t>(row), unused)] =
+              s_vec[511] + part;
+        }
       }
     }
   }
@@ -361,6 +365,21 @@ static void magic_for(unsigned d, unsigned long long* magic, int* shift) {
   while ((1ull << s) < d) ++s;
   *magic = ((1ull << (31 + s)) / d) + 1;
   *shift = 31 + s;
+}
+
+// one instantiation per padded operator width (the host dispatches once per launch)
+template <int kN>
+static const char* launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, const SmemLayout& L,
+                          int grid, int E, uint32_t smem_bytes, cudaStream_t stream) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(dft_gemm_kernel<kN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+      return "cudaFuncSetAttribute(max dynamic smem) failed";
+    attr_set = true;
+  }
+  dft_gemm_kernel<kN><<<grid, 128 * E + 32, smem_bytes, stream>>>(tmA, tmB, p, L);
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
 const char* dft_gemm_launch(const void* A, long long lda, const void* Bmat, GemmParams p, int num_sms,
@@ -392,16 +411,15 @@ const char* dft_gemm_launch(const void* A, long long lda, const void* Bmat, Gemm
   if (p.epi.mode == EPI_ROWMAJOR && p.epi.vec_ok && p.N % 8 == 0 && (p.N == 8 || p.N == 16 || p.N == 32 ||
       p.N == 64 || p.N == 128 || p.N == 256))
     pitch = ((p.N + 15) / 16 * 16) * (p.epi.out_fp32 ? 4 : 2) + 16;   // whole 16-column chunks are staged
-  // consumer warpgroups, staging, ring depth and K chunk: two warpgroups with >= 2 whole-K stages each if possible;
-  // for long K the largest divisor of the K blocks that leaves room for two stages
+  // consumer warpgroups, staging, ring depth and K chunk: as many warpgroups as the accumulator allows with >= 2
+  // stages each, whole-K stages if possible, else the largest divisor of the K blocks that leaves room for two
   bool ok = false;
-  int E = kMaxGroups;
+  int E = dft_max_groups(p.n_pad);
   for (; E >= 1 && !ok; --E) {
     for (int with_stage = pitch ? 1 : 0; with_stage >= 0 && !ok; --with_stage) {
-      const uint32_t scratch = 4u * E * kRowScratchFloats * 4;
       const uint32_t stg = with_stage ? 4u * E * 32 * pitch : 0;
-      if (fixed + scratch + stg > 227 * 1024) continue;
-      const uint32_t avail = 227 * 1024 - fixed - scratch - stg;
+      if (fixed + stg > 227 * 1024) continue;
+      const uint32_t avail = 227 * 1024 - fixed - stg;
       for (int dv = kblocks; dv >= 1 && !ok; --dv) {
         if (kblocks % dv) continue;
         const uint32_t a_tile = static_cast<uint32_t>(dv) * tile_m * 128;
@@ -410,8 +428,7 @@ const char* dft_gemm_launch(const void* A, long long lda, const void* Bmat, Gemm
         if (spg >= 2) {
           L.kbs = static_cast<uint32_t>(dv); L.a_tile_bytes = a_tile; L.spg = spg;
           L.stage_pitch = with_stage ? pitch : 0;
-          L.scratch_off = L.b_bytes + E * spg * a_tile + 4096;
-          L.stage_off = L.scratch_off + scratch;
+          L.stage_off = L.b_bytes + E * spg * a_tile + 4096;
           ok = true;
         }
       }
@@ -433,19 +450,26 @@ const char* dft_gemm_launch(const void* A, long long lda, const void* Bmat, Gemm
                   static_cast<uint64_t>(p.k_pad), kBlockK, static_cast<uint32_t>(p.n_pad)))
     return "cuTensorMapEncodeTiled(B) failed";
 
-  static bool attr_set[2] = {false, false};
-  const void* fn = halves == 2 ? reinterpret_cast<const void*>(dft_gemm_kernel<2>) : reinterpret_cast<const void*>(dft_gemm_kernel<1>);
-  if (!attr_set[halves - 1]) {
-    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-      return "cudaFuncSetAttribute(max dynamic smem) failed";
-    attr_set[halves - 1] = true;
-  }
   const int num_tiles = static_cast<int>((p.M + tile_m - 1) / tile_m);
   const int grid = num_tiles < num_sms ? num_tiles : num_sms;
-  if (halves == 2) dft_gemm_kernel<2><<<grid, 128 * E + 32, smem_bytes, stream>>>(tmA, tmB, p, L);
-  else dft_gemm_kernel<1><<<grid, 128 * E + 32, smem_bytes, stream>>>(tmA, tmB, p, L);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+  switch (p.n_pad) {
+    case 16: return launch<16>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 32: return launch<32>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 48: return launch<48>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 64: return launch<64>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 80: return launch<80>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 96: return launch<96>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 112: return launch<112>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 128: return launch<128>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 144: return launch<144>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 160: return launch<160>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 176: return launch<176>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 192: return launch<192>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 208: return launch<208>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 224: return launch<224>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    case 240: return launch<240>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+    default: return launch<256>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
+  }
 }
 
 }  // namespace dfno

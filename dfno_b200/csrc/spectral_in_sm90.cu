@@ -61,32 +61,6 @@ __device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, const void* s
                : "memory");
 }
 
-// D = A . B^T over `kblocks` >= 1 K blocks of 64 (four k16 steps each), both operands K-major (a_blk / b_blk bytes
-// per block), N columns and kHalves m64 halves (rows 64..127 into acc[R/2, R)).  N and kHalves are compile-time
-// constants and the k16 steps of a block are unrolled, so that the chain's wgmmas issue back to back with one commit
-// and one wait: a width chosen per instruction makes ptxas serialise every wgmma (C7511), and a fully unrolled
-// K loop runs out of (uniform) registers for the descriptors and is serialised too.  The block loop is a run-time
-// loop with a fence per block; ptxas closes it with one extra arrive before the wait (C7519).
-template <int N, int kHalves, int R>
-__device__ __forceinline__ void mma_chain(float (&acc)[R], uint32_t a, uint32_t a_blk, uint32_t b, uint32_t b_blk,
-                                          int kblocks) {
-  int kb = 0;
-#pragma unroll 1
-  do {
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      const uint64_t da = gdesc_k128(a + kb * a_blk + kk * 32), db = gdesc_k128(b + kb * b_blk + kk * 32);
-      const uint32_t scale_d = kb > 0 || kk > 0 ? 1u : 0u;
-      wg_mma64<false, 0, 0, 0>(acc, N, da, db, scale_d);
-      if constexpr (kHalves == 2) wg_mma64<false, 0, 0, R / 2>(acc, N, da + (8192 >> 4), db, scale_d);
-    }
-  } while (++kb < kblocks);
-  wgmma_commit();
-  wgmma_wait<0>();
-  acc_fence(acc);
-}
-
 // One dispatch per chain (never per instruction) on the tile rows; the second m64 half is skipped when the tile has
 // at most 64 rows (its A rows would lie past the operand block).
 template <int N, int R>

@@ -26,9 +26,10 @@ def pad_operator(B: torch.Tensor, device=None) -> torch.Tensor:
 
 
 # Shared-memory sizing of dft_gemm_launch (csrc/dft_gemm_sm90.cu); keep the two in step.  The padded operator stays
-# resident next to 5 KB of barriers, tables and alignment slack, the row scratch of one consumer warpgroup
-# (4 warps x kRowScratchFloats = 32 x 17 floats) and a ring of at least two A stages of one 64-wide K block each
-# (64 rows when n_pad > 128, else 128).  Any other configuration the launcher tries needs more.
+# resident next to 5 KB of barriers, tables and alignment slack and a ring of at least two A stages of one 64-wide
+# K block each (64 rows when n_pad > 128, else 128).  The formula also counts 8.5 KB of per-warp row scratch that the
+# kernel no longer uses (its epilogues work on the accumulator fragments), so every shape admitted here launches with
+# room to spare; the smallest configuration the launcher tries is the one above.
 DFT_GEMM_SMEM = 227 * 1024
 
 
