@@ -16,6 +16,16 @@
 //                                 loss gradient inside the fp16 range; undone when the sums are flushed)
 //             MMA2  dh0[pos, i]    = sum_j P[pos, j] W3[j, i]          epi B: g[i, pos] = dout[pos] dh0[pos, i]
 //             MMA3  D3[j, i]      += sum_pos P[pos, j] hs[i, pos]      -> dW3 (i < C), db3 (i = C)
+//
+// Widths 48 and 64 (KR = 64, 80): W3aug spans KR columns, so at KR = 80 it is two 64-column swizzle blocks ([H, 128]
+// in memory, b3 in column 64).  The backward cannot hold dh0 (KR registers), D3 (KR) and an MMA1 half (64) at once in
+// the 240 registers of a consumer: it runs MMA2 after both MMA1 halves, from the P tile in shared memory, in two
+// channel-column groups (32 + 32 or 48 + 32) whose epilogue B runs in turn.  MMA1 runs in 32-unit quarters, the hs
+// copy walks its four rows in a loop (unrolled, ptxas keeps all 4 KR of its shared addresses live across tiles), the
+// dW4 sums stay in shared memory as at KR = 48 (24 of the 32 at KR = 80), and g is staged in the warpgroup's hs buffer
+// (free once MMA3 has read it), which keeps KR = 80 inside shared memory.
+#include <type_traits>
+
 #include "head_common.cuh"
 #include "kernels.h"
 #include "tma_host.h"
@@ -45,8 +55,9 @@ __global__ void __launch_bounds__(kThreadsHF, 1)
 head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
                 const HeadFwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* s_w3 = smem;                                    // [128 hid][64] K-major, column C = b3
-  uint8_t* s_a = smem + 16384;                             // stages x 2 halves x [KR rows][64 pos]
+  constexpr uint32_t w3_bytes = KR > 64 ? 32768u : 16384u;  // one or two [128 hid][64] blocks
+  uint8_t* s_w3 = smem;                                    // [128 hid][64] K-major block(s), column C = b3
+  uint8_t* s_a = smem + w3_bytes;                          // stages x 2 halves x [KR rows][64 pos]
   constexpr uint32_t half_bytes = KR * 128;
   constexpr uint32_t stage_bytes = 2 * half_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_a + kStagesHF * stage_bytes);
@@ -80,8 +91,9 @@ head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__
 
   if (warp == 4 * kGroupsHF) {
     if (lane == 0) {
-      mbar_arrive_expect_tx(wfull, 16384);
+      mbar_arrive_expect_tx(wfull, w3_bytes);
       tma_load_2d(s_w3, &tmW3, wfull, 0, 0);
+      if constexpr (KR > 64) tma_load_2d(s_w3 + 16384, &tmW3, wfull, 64, 0);
       uint32_t s = 0, ph = 0;
       for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int b = static_cast<int>(tile / p.tiles_per_b);
@@ -116,9 +128,12 @@ head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__
     const uint32_t abase = smem_u32(s_a + s * stage_bytes);
     wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < KR / 16; ++ks)
+    for (int ks = 0; ks < KR / 16; ++ks) {
+      // k16 step ks of W3aug: 64-column block ks / 4 (a second block only at KR = 80)
+      const uint32_t w_k = KR > 64 ? (ks >> 2) * 16384 + (ks & 3) * 32 : ks * 32;
       wg_mma128<false, 1, 0>(acc, kHidH, gdesc_mn128(abase + ks * 2048, half_bytes, 1024), half_bytes,
-                             gdesc_k128(w_addr + ks * 32), ks > 0 ? 1u : 0u);
+                             gdesc_k128(w_addr + w_k), ks > 0 ? 1u : 0u);
+    }
     wgmma_commit();
     wgmma_wait<0>();
     acc_fence(acc);
@@ -154,8 +169,15 @@ constexpr int kGroupsHB = 2;                    // consumer warpgroups (stages a
 constexpr int kThreadsHB = 128 * kGroupsHB + 128;
 constexpr int kProducerRegsHB = 24, kConsumerRegsHB = 240;
 static_assert(128 * kProducerRegsHB + 128 * kGroupsHB * kConsumerRegsHB <= 65536, "register file");
+// KR = 64, 80 (widths 48, 64): MMA2 from shared memory in channel groups, g staged over hs (see the file header)
 template <int KR>
-constexpr bool kWsumSmem = KR > 32;
+constexpr bool kWideHB = KR > 48;
+template <int KR>
+constexpr bool kWsumSmem = KR > 32 && !kWideHB<KR>;
+// KR = 64, 80: the first kWsumSmemW dW4 column sums live in shared memory, the rest in registers (all 32 do not fit the
+// shared memory of KR = 80)
+template <int KR>
+constexpr int kWsumSmemW = !kWideHB<KR> ? 0 : KR > 64 ? 24 : 32;
 
 struct HeadBwdParams {
   int B, C, KR, stages;
@@ -181,15 +203,18 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr uint32_t half_bytes = KR * 128;
   constexpr uint32_t tile_bytes = 2 * half_bytes;
-  uint8_t* s_w3 = smem;                                   // 16 KB
-  uint8_t* s_w3t = s_w3 + 16384;                          // 2 k-blocks x [KR c rows][64 hid] fp16
+  constexpr uint32_t w3_bytes = KR > 64 ? 32768u : 16384u;
+  uint8_t* s_w3 = smem;                                   // 16 KB (32 KB at KR = 80)
+  uint8_t* s_w3t = s_w3 + w3_bytes;                       // 2 k-blocks x [KR c rows][64 hid] fp16
   uint8_t* s_p = s_w3t + tile_bytes;                      // per warpgroup: 2 x [128 pos][64 hid] fp16
   uint8_t* s_a = s_p + kGroupsHB * 32768;                 // stages x h tile
   uint8_t* s_hs = s_a + p.stages * tile_bytes;            // per warpgroup: scaled fp16 copy of the h tile
-  uint8_t* s_g = s_hs + kGroupsHB * tile_bytes;           // per warpgroup: bf16 g staging, 2 x [KR c rows][64 pos]
+  // per warpgroup: bf16 g staging, 2 x [KR c rows][64 pos] (the hs buffer itself at KR >= 64)
+  uint8_t* s_g = kWideHB<KR> ? s_hs : s_hs + kGroupsHB * tile_bytes;
   // KR = 48 leaves no registers for the dW4 column sums: they live in [32][consumer threads] floats instead
   float* s_wsum = reinterpret_cast<float*>(s_g + kGroupsHB * tile_bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_wsum + (kWsumSmem<KR> ? 32 * 128 * kGroupsHB : 0));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_wsum + (kWsumSmem<KR> ? 32 * 128 * kGroupsHB : 0) +
+                                               kWsumSmemW<KR> * 128 * kGroupsHB);
   uint64_t* a_full = bars;            // [8]
   uint64_t* a_empty = bars + 8;       // [8]
   uint64_t* w_full = bars + 16;
@@ -226,8 +251,9 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
   if (warp >= 4 * kGroupsHB) {
     setmaxnreg_dec<kProducerRegsHB>();
     if (warp == 4 * kGroupsHB && lane == 0) {
-      mbar_arrive_expect_tx(w_full, 16384 + tile_bytes);
+      mbar_arrive_expect_tx(w_full, w3_bytes + tile_bytes);
       tma_load_2d(s_w3, &tmW3, w_full, 0, 0);
+      if constexpr (KR > 64) tma_load_2d(s_w3 + 16384, &tmW3, w_full, 64, 0);
       tma_load_2d(s_w3t, &tmW3T, w_full, 0, 0);
       tma_load_2d(s_w3t + half_bytes, &tmW3T, w_full, 64, 0);
       uint32_t s = 0, ph = 0;
@@ -267,23 +293,60 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
 #pragma unroll
   for (int i = 0; i < 32; ++i) {
     if constexpr (kWsumSmem<KR>) my_wsum[i * 128 * kGroupsHB] = 0.f;
+    else if constexpr (kWideHB<KR>) { if (i < kWsumSmemW<KR>) my_wsum[i * 128 * kGroupsHB] = 0.f; else wsum[i] = 0.f; }
     else wsum[i] = 0.f;
   }
   // dW4 column sum i += v
   auto wsum_add = [&](int i, float d, float v) {
     if constexpr (kWsumSmem<KR>) my_wsum[i * 128 * kGroupsHB] = fmaf(d, v, my_wsum[i * 128 * kGroupsHB]);
-    else wsum[i] = fmaf(d, v, wsum[i]);
+    else if constexpr (kWideHB<KR>) {
+      if (i < kWsumSmemW<KR>) my_wsum[i * 128 * kGroupsHB] = fmaf(d, v, my_wsum[i * 128 * kGroupsHB]);
+      else wsum[i] = fmaf(d, v, wsum[i]);
+    } else wsum[i] = fmaf(d, v, wsum[i]);
   };
   float d3[KR];                                      // [hid, c] over this warpgroup's tiles: 128 x KR
   uint32_t pa[2][4][4];                              // P of one 64-unit hidden half: [m64 half][k16 step][A register]
   // MMA2, hidden units [64 kb, 64 kb + 64): dh0 (+)= P . W3, A = the P registers
   auto mma2 = [&](float (&acc2)[KR], int kb) {
+    if constexpr (!kWideHB<KR>) {
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      const uint64_t db = gdesc_k128(w3t_addr + kb * half_bytes + ks * 32);
-      const uint32_t sc = (kb > 0 || ks > 0) ? 1u : 0u;
-      wg_mma64_rs<KR, 0, 0>(acc2, pa[0][ks], db, sc);
-      wg_mma64_rs<KR, 0, KR / 2>(acc2, pa[1][ks], db, sc);
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint64_t db = gdesc_k128(w3t_addr + kb * half_bytes + ks * 32);
+        const uint32_t sc = (kb > 0 || ks > 0) ? 1u : 0u;
+        wg_mma64_rs<KR, 0, 0>(acc2, pa[0][ks], db, sc);
+        wg_mma64_rs<KR, 0, KR / 2>(acc2, pa[1][ks], db, sc);
+      }
+    }
+  };
+  // KR >= 64: MMA2 for the channel columns [c0, c0 + NG), A = the P tile in shared memory (K-major, hidden units
+  // contiguous), then epilogue B of those columns into the g staging
+  auto mma2_group = [&](auto c0_, auto ng_, const float (&dk)[4]) {
+    constexpr int c0 = decltype(c0_)::value, NG = decltype(ng_)::value;
+    float a2[NG];                                    // dh0 [pos, c0 + n]: 128 x NG
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      const uint32_t kb = ks >> 2, kk = ks & 3;
+      wg_mma128<true, 0, 0>(a2, NG, gdesc_k128(p_addr + kb * 16384 + kk * 32), 8192,
+                            gdesc_k128(w3t_addr + kb * half_bytes + c0 * 128 + kk * 32), ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(a2);
+#pragma unroll
+    for (int mh = 0; mh < 2; ++mh) {
+#pragma unroll
+      for (int t = 0; t < NG / 16; ++t) {
+        uint32_t r[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float* a = a2 + (NG / 2) * mh + 4 * (2 * t + (i >> 1)) + 2 * (i & 1);
+          const float d = dk[2 * mh + (i & 1)];
+          r[i] = pack_bf16x2(d * a[0], d * a[1]);
+        }
+        const uint32_t c = c0 + 16 * t + 8 * (mi >> 1) + mk;
+        stmatrix_x4_trans(g_addr + mh * half_bytes + c * 128 + ((g_chunk ^ (c & 7)) << 4), r);
+      }
     }
   };
   long long n = 0, mine = 0;
@@ -301,42 +364,130 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
     for (int k = 0; k < 4; ++k) dk[k] = __shfl_sync(0xffffffffu, dl, (lane & ~3) | k);
     mbar_wait(&a_full[s], (n / p.stages) & 1);
     const uint32_t abase = smem_u32(s_a + s * tile_bytes);
-    float acc2[KR];                                  // dh0 [pos, c]: 128 x KR
+    float acc2[KR];                                  // dh0 [pos, c]: 128 x KR (KR <= 48)
+    if constexpr (kWideHB<KR>) {
+      // MMA1 in four 32-unit quarters (the registers of a 64-unit half are taken by D3); P goes to shared memory only
 #pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {                 // hidden units [64 hh, 64 hh + 64)
-      float acc[64];
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < KR / 16; ++ks)
-        wg_mma128<false, 1, 0>(acc, 64, gdesc_mn128(abase + ks * 2048, half_bytes, 1024), half_bytes,
-                               gdesc_k128(w3_addr + hh * 8192 + ks * 32), ks > 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      acc_fence(acc);
-      // ---- epi A: P = W4 gelu'(pre) into the A registers and the smem tile; dW4 += dout gelu(pre)
-#pragma unroll
-      for (int mh = 0; mh < 2; ++mh) {
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          afrag_from_acc(acc + 32 * mh, ks, pa[mh][ks], [&](float lo, float hi, int i) {
-            const int j = 2 * ks + (i >> 1);
-            const GeluH2 vg = gelu_vg_h2(h2_from_f32(lo, hi));
-            const float2 a = __half22float2(vg.value);
-            const float d = dk[2 * mh + (i & 1)];
-            wsum_add(16 * hh + 2 * j, d, a.x);
-            wsum_add(16 * hh + 2 * j + 1, d, a.y);
-            return h2_bits(__hmul2(vg.grad, h2_of_bits(s_w4h[32 * hh + 4 * j + cq])));
-          });
-          const uint32_t row = 64 * mh + p_row, chunk = 2 * ks + (mi >> 1);
-          stmatrix_x4(p_addr + hh * 16384 + row * 128 + ((chunk ^ (row & 7)) << 4), pa[mh][ks]);
-        }
-      }
-      if (hh == 0) {                                 // MMA2 over the first half, before the second half's MMA1
+      for (int hq = 0; hq < 4; ++hq) {               // hidden units [32 hq, 32 hq + 32)
+        float acc[32];
         wgmma_fence();
-        mma2(acc2, 0);
+#pragma unroll
+        for (int ks = 0; ks < KR / 16; ++ks) {
+          const uint32_t w_k = KR > 64 ? (ks >> 2) * 16384 + (ks & 3) * 32 : ks * 32;
+          wg_mma128<false, 1, 0>(acc, 32, gdesc_mn128(abase + ks * 2048, half_bytes, 1024), half_bytes,
+                                 gdesc_k128(w3_addr + hq * 4096 + w_k), ks > 0 ? 1u : 0u);
+        }
         wgmma_commit();
         wgmma_wait<0>();
+        acc_fence(acc);
+        const int hh = hq >> 1;
+#pragma unroll
+        for (int mh = 0; mh < 2; ++mh) {
+#pragma unroll
+          for (int kq = 0; kq < 2; ++kq) {
+            const int ks = 2 * (hq & 1) + kq;            // k16 step inside the 64-unit half hh (epi A as below)
+            uint32_t pr[4];
+            afrag_from_acc(acc + 16 * mh, kq, pr, [&](float lo, float hi, int i) {
+              const int j = 2 * ks + (i >> 1);
+              const GeluH2 vg = gelu_vg_h2(h2_from_f32(lo, hi));
+              const float2 a = __half22float2(vg.value);
+              const float d = dk[2 * mh + (i & 1)];
+              wsum_add(16 * hh + 2 * j, d, a.x);
+              wsum_add(16 * hh + 2 * j + 1, d, a.y);
+              return h2_bits(__hmul2(vg.grad, h2_of_bits(s_w4h[32 * hh + 4 * j + cq])));
+            });
+            const uint32_t row = 64 * mh + p_row, chunk = 2 * ks + (mi >> 1);
+            stmatrix_x4(p_addr + hh * 16384 + row * 128 + ((chunk ^ (row & 7)) << 4), pr);
+          }
+        }
       }
+    } else {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {                 // hidden units [64 hh, 64 hh + 64)
+        float acc[64];
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < KR / 16; ++ks)
+          wg_mma128<false, 1, 0>(acc, 64, gdesc_mn128(abase + ks * 2048, half_bytes, 1024), half_bytes,
+                                 gdesc_k128(w3_addr + hh * 8192 + ks * 32), ks > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        acc_fence(acc);
+        // ---- epi A: P = W4 gelu'(pre) into the A registers and the smem tile; dW4 += dout gelu(pre)
+#pragma unroll
+        for (int mh = 0; mh < 2; ++mh) {
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {
+            afrag_from_acc(acc + 32 * mh, ks, pa[mh][ks], [&](float lo, float hi, int i) {
+              const int j = 2 * ks + (i >> 1);
+              const GeluH2 vg = gelu_vg_h2(h2_from_f32(lo, hi));
+              const float2 a = __half22float2(vg.value);
+              const float d = dk[2 * mh + (i & 1)];
+              wsum_add(16 * hh + 2 * j, d, a.x);
+              wsum_add(16 * hh + 2 * j + 1, d, a.y);
+              return h2_bits(__hmul2(vg.grad, h2_of_bits(s_w4h[32 * hh + 4 * j + cq])));
+            });
+            const uint32_t row = 64 * mh + p_row, chunk = 2 * ks + (mi >> 1);
+            stmatrix_x4(p_addr + hh * 16384 + row * 128 + ((chunk ^ (row & 7)) << 4), pa[mh][ks]);
+          }
+        }
+        if (hh == 0) {                                 // MMA2 over the first half, before the second half's MMA1
+          wgmma_fence();
+          mma2(acc2, 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+        }
+      }
+    }
+    if constexpr (kWideHB<KR>) {
+      if (leader) tma_store_wait_read();             // hs doubles as the g staging: the previous g stores must be out
+      asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
+      const uint8_t* src = s_a + s * tile_bytes;     // hs as below, one row per iteration
+#pragma unroll 1
+      for (int k = 0; k < 4; ++k) {
+        const int row = frag_row(q, lane, k);
+        const float ds = dk[k] * scale;
+        const uint32_t colo = (row >> 6) * half_bytes + ((row & 7) << 1);
+        const uint32_t ch = (row & 63) >> 3;
+#pragma unroll
+        for (int cc = 0; cc < KR / 4; ++cc) {
+          const int c = 4 * cc + cq;
+          const uint32_t off = colo + c * 128 + ((ch ^ (c & 7)) << 4);
+          if (c < p.C) {
+            const uint16_t hv = *reinterpret_cast<const uint16_t*>(src + off);
+            *reinterpret_cast<__half*>(hsbuf + off) = __float2half_rn(__uint_as_float(static_cast<uint32_t>(hv) << 16) * ds);
+          } else if (c == p.C) {
+            *reinterpret_cast<__half*>(hsbuf + off) = __float2half_rn(ds);
+          }
+        }
+      }
+
+      fence_proxy_async_smem();
+      asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
+      if (leader) mbar_arrive(&a_empty[s]);          // the h tile has been read for the last time
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) {
+        const uint32_t kb = ks >> 2, kk = ks & 3;
+        wg_mma128<true, 1, 0>(d3, KR, gdesc_mn128(p_addr + ks * 2048, 16384, 1024), 16384,
+                              gdesc_k128(hs_addr + kb * half_bytes + kk * 32), (mine > 0 || ks > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();                               // MMA3 has read hs before g is staged over it
+      acc_fence(d3);
+      ++mine;
+      constexpr int kG0 = KR > 64 ? 48 : 32;         // channel columns of the first MMA2 group
+      mma2_group(std::integral_constant<int, 0>{}, std::integral_constant<int, kG0>{}, dk);
+      mma2_group(std::integral_constant<int, kG0>{}, std::integral_constant<int, KR - kG0>{}, dk);
+      fence_proxy_async_smem();
+      asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
+      if (leader) {
+        const int row0 = b * p.C;
+        tma_store_2d(&tmG, gbuf, static_cast<int32_t>(p0), row0);
+        if (p0 + 64 < p.S) tma_store_2d(&tmG, gbuf + half_bytes, static_cast<int32_t>(p0 + 64), row0);
+        tma_store_commit();
+      }
+      continue;
     }
     {
       // ---- hs: scaled fp16 copy of the h tile at the thread's rows, channels c = l%4 (mod 4); row C = the scaled
@@ -359,7 +510,7 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
             *reinterpret_cast<__half*>(hsbuf + off) = __float2half_rn(ds);
           }
         }
-      }
+    }
     }
     if (leader) tma_store_wait_read();               // the previous tile's g staging is free after the barrier
     fence_proxy_async_smem();
@@ -413,7 +564,7 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
   if (lane == 0) atomicAdd(s_gb4, acc_gb4);
 #pragma unroll
   for (int i = 0; i < 32; ++i) {                     // lanes with equal l%4 hold the same hidden units
-    float v = kWsumSmem<KR> ? my_wsum[i * 128 * kGroupsHB] : wsum[i];
+    float v = kWsumSmem<KR> || i < kWsumSmemW<KR> ? my_wsum[i * 128 * kGroupsHB] : wsum[i];
     v += __shfl_xor_sync(0xffffffffu, v, 4);
     v += __shfl_xor_sync(0xffffffffu, v, 8);
     v += __shfl_xor_sync(0xffffffffu, v, 16);
@@ -446,11 +597,11 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
 
 }  // namespace
 
-// h: bf16 [B*C, S] channel-major; W3aug: bf16 [128, 64] with column C = b3; w4b4: fp32 [129]; out: fp32, addressed
+// h: bf16 [B*C, S] channel-major; W3aug: bf16 [128, 64] with column C = b3 ([128, 128] when C = 64); w4b4: fp32 [129]; out: fp32, addressed
 // through the row digits (row = b*S + position).
 const char* head_fwd(const void* h, const void* W3aug, const float* w4b4, float* out, int B, int C, long long S,
                      int nrl, const int* R, const long long* SR, int num_sms, cudaStream_t stream) {
-  if (C < 1 || C > 47) return "head_fwd: 1 <= C <= 47";
+  if (C < 1 || C > 64) return "head_fwd: 1 <= C <= 64";
   if (S % 8 || S > (1ll << 31) - 256 || static_cast<long long>(B) * S > (1ll << 31) - 256) return "head_fwd: bad slab size";
   HeadFwdParams p{};
   p.B = B; p.C = C; p.KR = (C + 1 + 15) / 16 * 16; p.S = S; p.tiles_per_b = (S + 127) / 128;
@@ -458,23 +609,29 @@ const char* head_fwd(const void* h, const void* W3aug, const float* w4b4, float*
   if (set_rowmap(&p.map, nrl, R, SR)) return "head_fwd: 1..4 row digits";
   CUtensorMap tmH, tmW3;
   if (make_map_2d(&tmH, h, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (h) failed";
-  if (make_map_2d(&tmW3, W3aug, 64, 128, 64, 64, 128)) return "tensor map (W3) failed";
-  static bool attr[3] = {false, false, false};
+  const int w3_cols = p.KR > 64 ? 128 : 64;
+  if (make_map_2d(&tmW3, W3aug, w3_cols, 128, w3_cols, 64, 128)) return "tensor map (W3) failed";
+  static bool attr[5] = {false, false, false, false, false};
   const int kr_i = p.KR / 16 - 1;
-  const void* fn = kr_i == 0 ? reinterpret_cast<const void*>(head_fwd_kernel<16>)
-                 : kr_i == 1 ? reinterpret_cast<const void*>(head_fwd_kernel<32>)
-                             : reinterpret_cast<const void*>(head_fwd_kernel<48>);
+  const void* fns[5] = {reinterpret_cast<const void*>(head_fwd_kernel<16>),
+                        reinterpret_cast<const void*>(head_fwd_kernel<32>),
+                        reinterpret_cast<const void*>(head_fwd_kernel<48>),
+                        reinterpret_cast<const void*>(head_fwd_kernel<64>),
+                        reinterpret_cast<const void*>(head_fwd_kernel<80>)};
+  const void* fn = fns[kr_i];
   if (!attr[kr_i]) {
     if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
       return "cudaFuncSetAttribute failed";
     attr[kr_i] = true;
   }
-  const uint32_t smem_bytes = 16384 + kStagesHF * 2 * p.KR * 128 + 2048 + 1024;
+  const uint32_t smem_bytes = (p.KR > 64 ? 32768 : 16384) + kStagesHF * 2 * p.KR * 128 + 2048 + 1024;
   const long long tiles = p.tiles_per_b * B;
   const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
   if (kr_i == 0) head_fwd_kernel<16><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
   else if (kr_i == 1) head_fwd_kernel<32><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
-  else head_fwd_kernel<48><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
+  else if (kr_i == 2) head_fwd_kernel<48><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
+  else if (kr_i == 3) head_fwd_kernel<64><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
+  else head_fwd_kernel<80><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
@@ -485,7 +642,7 @@ const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const
                       long long n_dout, unsigned* amax_ws, void* g, float* gW3, float* gb3, float* gW4, float* gb4,
                       int B, int C, long long S, int nrl, const int* R, const long long* SR, int num_sms,
                       cudaStream_t stream) {
-  if (C < 1 || C > 32) return "head_bwd: 1 <= C <= 32";
+  if (C < 1 || C > 64) return "head_bwd: 1 <= C <= 64";
   if (S % 8 || S > (1ll << 31) - 256 || static_cast<long long>(B) * S > (1ll << 31) - 256) return "head_bwd: bad slab size";
   HeadBwdParams p{};
   p.B = B; p.C = C; p.KR = (C + 1 + 15) / 16 * 16; p.S = S; p.tiles_per_b = (S + 127) / 128;
@@ -494,14 +651,18 @@ const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const
   if (set_rowmap(&p.map, nrl, R, SR)) return "head_bwd: 1..4 row digits";
   CUtensorMap tmH, tmW3, tmW3T, tmG;
   if (make_map_2d(&tmH, h, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (h) failed";
-  if (make_map_2d(&tmW3, W3aug, 64, 128, 64, 64, 128)) return "tensor map (W3) failed";
+  const int w3_cols = p.KR > 64 ? 128 : 64;
+  if (make_map_2d(&tmW3, W3aug, w3_cols, 128, w3_cols, 64, 128)) return "tensor map (W3) failed";
   if (make_map_2d(&tmW3T, W3T16, 128, p.KR, 128, 64, p.KR)) return "tensor map (W3T) failed";
   if (make_map_2d(&tmG, g, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (g) failed";
-  static bool attr[3] = {false, false, false};
+  static bool attr[5] = {false, false, false, false, false};
   const int kr_i = p.KR / 16 - 1;
-  const void* fn = kr_i == 0 ? reinterpret_cast<const void*>(head_bwd2_kernel<16>)
-                 : kr_i == 1 ? reinterpret_cast<const void*>(head_bwd2_kernel<32>)
-                             : reinterpret_cast<const void*>(head_bwd2_kernel<48>);
+  const void* fns[5] = {reinterpret_cast<const void*>(head_bwd2_kernel<16>),
+                        reinterpret_cast<const void*>(head_bwd2_kernel<32>),
+                        reinterpret_cast<const void*>(head_bwd2_kernel<48>),
+                        reinterpret_cast<const void*>(head_bwd2_kernel<64>),
+                        reinterpret_cast<const void*>(head_bwd2_kernel<80>)};
+  const void* fn = fns[kr_i];
   if (!attr[kr_i]) {
     if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
       return "cudaFuncSetAttribute failed";
@@ -510,16 +671,21 @@ const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const
   if (cudaMemsetAsync(amax_ws, 0, 4, stream) != cudaSuccess) return "head_bwd: memset failed";
   absmax_kernel<<<num_sms * 4, 256, 0, stream>>>(dout, n_dout, amax_ws);
   const uint32_t tile_bytes = 2u * p.KR * 128;
-  const uint32_t fixed = 16384 + tile_bytes + kGroupsHB * (32768 + 2 * tile_bytes) + 2048 + 1024 +
-                         (p.KR > 32 ? 32 * 128 * kGroupsHB * 4 : 0);
+  const bool wide = p.KR > 48;                                     // g staged over hs
+  const uint32_t wsum_n = !wide ? (p.KR > 32 ? 32 : 0) : p.KR > 64 ? 24 : 32;   // dW4 sums in shared memory
+  const uint32_t fixed = (p.KR > 64 ? 32768 : 16384) + tile_bytes + kGroupsHB * (32768 + (wide ? 1 : 2) * tile_bytes) +
+                         2048 + 1024 + wsum_n * 128 * kGroupsHB * 4;
   p.stages = kMaxStagesHB;
   while (p.stages > kGroupsHB && fixed + p.stages * tile_bytes > 227 * 1024) p.stages -= kGroupsHB;
+  if (fixed + p.stages * tile_bytes > 227 * 1024) return "head_bwd: tile does not fit shared memory";
   const uint32_t smem_bytes = fixed + p.stages * tile_bytes;
   const long long tiles = p.tiles_per_b * B;
   const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
   if (kr_i == 0) head_bwd2_kernel<16><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
   else if (kr_i == 1) head_bwd2_kernel<32><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
-  else head_bwd2_kernel<48><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
+  else if (kr_i == 2) head_bwd2_kernel<48><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
+  else if (kr_i == 3) head_bwd2_kernel<64><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
+  else head_bwd2_kernel<80><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }

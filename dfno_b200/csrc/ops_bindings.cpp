@@ -300,7 +300,8 @@ void dpre_dw(const at::Tensor& g, at::Tensor& pre_dpre, const at::Tensor& h, at:
 void head_fwd(const at::Tensor& h, const at::Tensor& W3aug, const at::Tensor& w4b4, at::Tensor& out, int64_t B,
               int64_t C, int64_t S, const std::vector<int64_t>& radices, const std::vector<int64_t>& strides) {
   TORCH_CHECK(radices.size() == strides.size() && !radices.empty() && radices.size() <= 4, "1..4 row digits");
-  TORCH_CHECK(W3aug.dim() == 2 && W3aug.size(0) == 128 && W3aug.size(1) == 64 && W3aug.is_contiguous(), "W3aug [128,64]");
+  TORCH_CHECK(W3aug.dim() == 2 && W3aug.size(0) == 128 && W3aug.size(1) == (C + 1 > 64 ? 128 : 64) &&
+              W3aug.is_contiguous(), "W3aug [128, 64] ([128, 128] when C + 1 > 64)");
   TORCH_CHECK(w4b4.numel() >= 129, "w4b4 = [W4 (128), b4]");
   c10::cuda::CUDAGuard guard(h.device());
   int R[4]; long long SR[4];
@@ -314,7 +315,8 @@ void head_bwd2(const at::Tensor& h, const at::Tensor& W3aug, const at::Tensor& W
                at::Tensor& gW4, at::Tensor& gb4, int64_t B, int64_t C, int64_t S, const std::vector<int64_t>& radices,
                const std::vector<int64_t>& strides) {
   TORCH_CHECK(radices.size() == strides.size() && !radices.empty() && radices.size() <= 4, "1..4 row digits");
-  TORCH_CHECK(W3aug.dim() == 2 && W3aug.size(0) == 128 && W3aug.size(1) == 64 && W3aug.is_contiguous(), "W3aug [128,64]");
+  TORCH_CHECK(W3aug.dim() == 2 && W3aug.size(0) == 128 && W3aug.size(1) == (C + 1 > 64 ? 128 : 64) &&
+              W3aug.is_contiguous(), "W3aug [128, 64] ([128, 128] when C + 1 > 64)");
   TORCH_CHECK(W3T16.is_cuda() && W3T16.scalar_type() == at::kHalf && W3T16.dim() == 2 && W3T16.size(1) == 128 &&
               W3T16.size(0) == (C + 1 + 15) / 16 * 16 && W3T16.is_contiguous(), "W3T16: fp16 [ceil16(C+1), 128]");
   TORCH_CHECK(amax_ws.is_cuda() && amax_ws.numel() >= 1 && amax_ws.element_size() == 4, "amax_ws: one 32-bit word");

@@ -147,14 +147,19 @@ lift_fwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
 // owns z0 + 2cg and z0 + 2cg + 1, whose 2 * Tin values are contiguous in x's layout and written by this lane alone:
 // no atomics, no memset.  Tin == 1 keeps the 2 * CIN sums in registers over t; otherwise the first t stores and
 // later t add (read-modify-write of the lane's own run, which stays in L1 / L2).
+//
+// Widths above 32 (48, 64) split the channels over eight lanes instead (kSplit): each lane keeps C/8 channel sums, the
+// per-thread register cost of width 32.  The input gradient is then written by the first four lanes of the eight.
 template <typename TIn, int C, int CIN, bool kRegs, bool kDx>
 __global__ void __launch_bounds__(128, (CIN == 1 ? 4 : 2))      // several input channels: more live values, no spills
 lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
                 const float* __restrict__ W2, const float* __restrict__ b2,
                 const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
                 float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx) {
-  static_assert(C % 4 == 0, "the channels are split over four lanes");
-  constexpr int CG = C / 4;
+  constexpr int kSplitLog = C > 32 ? 3 : 2;
+  constexpr int kSplit = 1 << kSplitLog;                     // lanes per item
+  static_assert(C % kSplit == 0, "the channels are split evenly over the lanes of an item");
+  constexpr int CG = C / kSplit;
   __shared__ float sw[kLiftMaxW];
   __shared__ float sg[kLiftMaxW];
   float* sW1 = sw;
@@ -178,13 +183,14 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
     for (int ci = 0; ci < CIN; ++ci) accW2[u][ci] = 0.f;
   }
   const int lane = threadIdx.x & 31;
-  const int cg = lane & 3, c0 = cg * CG;                     // this lane's channels: [c0, c0 + CG)
+  const int cg = lane & (kSplit - 1), c0 = cg * CG;          // this lane's channels: [c0, c0 + CG)
+  const bool dx_lane = kSplit == 4 || cg < 4;                // lanes 0..3 of the item own its 8 z of dx
   const int zv = d.Z >> 3;
   const long long plane = static_cast<long long>(d.X) * d.Y;
   const long long nitems = static_cast<long long>(d.B) * plane * zv;
-  const long long per_it = (static_cast<long long>(gridDim.x) * blockDim.x) >> 2;
+  const long long per_it = (static_cast<long long>(gridDim.x) * blockDim.x) >> kSplitLog;
   const long long nloop = (nitems + per_it - 1) / per_it;
-  const long long item0 = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 2;
+  const long long item0 = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> kSplitLog;
   for (long long it = 0; it < nloop; ++it) {
     const long long idx = it * per_it + item0;
     const bool ok = idx < nitems;                           // whole warps stay in the loop (shuffles)
@@ -267,6 +273,7 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
           float v = da1[ci][z];
           v += __shfl_xor_sync(0xffffffffu, v, 1);
           v += __shfl_xor_sync(0xffffffffu, v, 2);
+          if constexpr (kSplit == 8) v += __shfl_xor_sync(0xffffffffu, v, 4);
           da1[ci][z] = v;
         }
       }
@@ -301,7 +308,7 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
           for (int z = 0; z < 8; ++z) sres = fmaf(e[z], xv[z], sres);
           sres = warp_sum(own ? sres : 0.f);
           if (lane == 0) atomicAdd(&gsW1[t * d.Tin + ti], sres);
-          if (kDx && !kRegs && ok) {
+          if (kDx && !kRegs && ok && dx_lane) {
             float* p = dxl + ci * xci_stride + ti;
             const float w = sW1[t * d.Tin + ti];
             if (t == 0) {
@@ -317,7 +324,7 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
       sb1v = warp_sum(own ? sb1v : 0.f);
       if (lane == 0) atomicAdd(&gsb1[t], sb1v);
     }
-    if (kDx && kRegs && ok) {
+    if (kDx && kRegs && ok && dx_lane) {
 #pragma unroll
       for (int ci = 0; ci < CIN; ++ci)
         *reinterpret_cast<float2*>(dxl + ci * xci_stride) = make_float2(dxr[ci][0], dxr[ci][1]);
@@ -326,9 +333,9 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
   __shared__ float gsW2[64 * 4 + 64];
   for (int i = threadIdx.x; i < C * CIN + C; i += blockDim.x) gsW2[i] = 0.f;
   __syncthreads();
-  // channel sums: lanes with the same quarter (lane & 3) hold partials of the same channels
+  // channel sums: lanes with the same share (lane % kSplit) hold partials of the same channels
   auto quarter_sum = [](float v) {
-    v += __shfl_xor_sync(0xffffffffu, v, 4);
+    if constexpr (kSplit == 4) v += __shfl_xor_sync(0xffffffffu, v, 4);
     v += __shfl_xor_sync(0xffffffffu, v, 8);
     v += __shfl_xor_sync(0xffffffffu, v, 16);
     return v;
@@ -336,11 +343,11 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
 #pragma unroll
   for (int u = 0; u < CG; ++u) {
     const float sres = quarter_sum(accb2[u]);
-    if (lane < 4) atomicAdd(&gsW2[C * CIN + c0 + u], sres);
+    if (lane < kSplit) atomicAdd(&gsW2[C * CIN + c0 + u], sres);
 #pragma unroll
     for (int ci = 0; ci < CIN; ++ci) {
       const float sw2 = quarter_sum(accW2[u][ci]);
-      if (lane < 4) atomicAdd(&gsW2[(c0 + u) * CIN + ci], sw2);
+      if (lane < kSplit) atomicAdd(&gsW2[(c0 + u) * CIN + ci], sw2);
     }
   }
   __syncthreads();
@@ -647,6 +654,14 @@ const char* lift_fwd(const void* x, int x_is_bf16, const float* W1, const float*
     default: return "unsupported channel width (supported: 4,8,12,16,20,24,32)"; \
   }
 
+// the lift backward's widths: those of every pointwise kernel, and 48 and 64 (the wide widths of the round-2 route)
+#define DFNO_LIFT_DISPATCH_C(C_, BODY)                \
+  switch (C_) {                                       \
+    case 48: { constexpr int kC = 48; BODY; } break;  \
+    case 64: { constexpr int kC = 64; BODY; } break;  \
+    default: DFNO_DISPATCH_C(C_, BODY)                \
+  }
+
 template <int C>
 static const char* lift_bwd_cin(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
                                 const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2,
@@ -679,10 +694,11 @@ const char* lift_bwd(const void* x, int x_is_bf16, const float* W1, const float*
   if (const char* e = lift_check(d)) return e;
   if (dx && reinterpret_cast<uintptr_t>(dx) % 8) return "lift_bwd: dx must be 8-byte aligned";
   const long long nitems = static_cast<long long>(d.B) * d.X * d.Y * (d.Z / 8);
-  const int grid = grid_for(4 * nitems, 128, num_sms, 4);          // four lanes per item (channel quarters)
+  const int split = d.C > 32 ? 8 : 4;                                 // lanes per item (see lift_bwd_kernel)
+  const int grid = grid_for(split * nitems, 128, num_sms, 4);
   const bool regs = d.Tin == 1;
   const char* err = nullptr;
-  DFNO_DISPATCH_C(d.C, (err = lift_bwd_cin<kC>(x, x_is_bf16, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, grid, regs,
+  DFNO_LIFT_DISPATCH_C(d.C, (err = lift_bwd_cin<kC>(x, x_is_bf16, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, grid, regs,
                                                s)));
   if (err) return err;
   cudaError_t e = cudaGetLastError();

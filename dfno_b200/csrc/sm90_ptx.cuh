@@ -208,7 +208,9 @@ DFNO_WGMMA(32, f16, DFNO_R2, 16, 17, 18, 19, 20, DFNO_F2)
 DFNO_WGMMA(48, bf16, DFNO_R3, 24, 25, 26, 27, 28, DFNO_F3)
 DFNO_WGMMA(48, f16, DFNO_R3, 24, 25, 26, 27, 28, DFNO_F3)
 DFNO_WGMMA(64, bf16, DFNO_R4, 32, 33, 34, 35, 36, DFNO_F4)
+DFNO_WGMMA(64, f16, DFNO_R4, 32, 33, 34, 35, 36, DFNO_F4)
 DFNO_WGMMA(80, bf16, DFNO_R5, 40, 41, 42, 43, 44, DFNO_F5)
+DFNO_WGMMA(80, f16, DFNO_R5, 40, 41, 42, 43, 44, DFNO_F5)
 DFNO_WGMMA(96, bf16, DFNO_R6, 48, 49, 50, 51, 52, DFNO_F6)
 DFNO_WGMMA(112, bf16, DFNO_R7, 56, 57, 58, 59, 60, DFNO_F7)
 DFNO_WGMMA(128, bf16, DFNO_R8, 64, 65, 66, 67, 68, DFNO_F8)
@@ -257,7 +259,8 @@ DFNO_WGMMA(256, bf16, DFNO_R16, 128, 129, 130, 131, 132, DFNO_F16)
 #undef DFNO_R16
 
 // acc[OFF .. OFF + n/2) (+)= A[64 x 16] . B[16 x n] for a run-time n (a multiple of 16); widths whose registers would
-// not fit between OFF and R are not instantiated.  kF16: fp16 inputs (the fp16 variants exist for n = 16, 32, 48, 128).
+// not fit between OFF and R are not instantiated.  kF16: fp16 inputs (the fp16 variants exist for n = 16, 32, 48, 64, 80
+// and 128).
 #define DFNO_WG_CASE(N)                                                                    \
   case N:                                                                                  \
     if constexpr (OFF + N / 2 <= R) wgmma_m64n##N##k16_bf16<TA, TB>(acc + OFF, da, db, scale_d); \
@@ -269,7 +272,10 @@ DFNO_WGMMA(256, bf16, DFNO_R16, 128, 129, 130, 131, 132, DFNO_F16)
 template <bool kF16, int TA, int TB, int OFF, int R>
 __device__ __forceinline__ void wg_mma64(float (&acc)[R], int n, uint64_t da, uint64_t db, uint32_t scale_d) {
   if constexpr (kF16) {
-    switch (n) { DFNO_WG_CASE16(16) DFNO_WG_CASE16(32) DFNO_WG_CASE16(48) DFNO_WG_CASE16(128) default: break; }
+    switch (n) {
+      DFNO_WG_CASE16(16) DFNO_WG_CASE16(32) DFNO_WG_CASE16(48) DFNO_WG_CASE16(64) DFNO_WG_CASE16(80)
+      DFNO_WG_CASE16(128) default: break;
+    }
   } else {
     switch (n) {
       DFNO_WG_CASE(16) DFNO_WG_CASE(32) DFNO_WG_CASE(48) DFNO_WG_CASE(64) DFNO_WG_CASE(80) DFNO_WG_CASE(96)

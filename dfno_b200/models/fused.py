@@ -42,9 +42,13 @@ from ..ops import operators as OPS
 from ..ops.gemm import DFT_GEMM_SMEM, ScatterSpec, dft_gemm_fits, dft_gemm_min_smem, pad_operator
 from ..parallel.partition import Partition
 
-__all__ = ["FusedDistributedFNO", "FusedAdam", "supports", "wants", "EnginePlan", "fold_onto_pencil"]
+__all__ = ["FusedDistributedFNO", "FusedAdam", "supports", "wants", "EnginePlan", "fold_onto_pencil",
+           "SUPPORTED_WIDTHS", "WIDE_WIDTHS"]
 
 SUPPORTED_WIDTHS = (4, 8, 12, 16, 20, 24, 32)
+# widths served by the round-2 route only (EnginePlan.fused_pw) with a single output channel: the wide-width spectral
+# mix, lift backward and channel-major head kernels exist for them, the round-1 kernels do not
+WIDE_WIDTHS = (48, 64)
 MAX_OUT = 4                  # output channels of the multi-output head kernels (csrc/head_multi_sm90.cu)
 MAX_N = 256                  # n_pad limit of dft_gemm (accumulator columns of one 64-row warpgroup tile)
 HBM_BUDGET = 72 * 2 ** 30    # of an H100's 80 GB: leave room for the CUDA context, NCCL and the allocator
@@ -121,8 +125,8 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
     B, Cin, X, Y, Z, Tin = shape6
     T = int(out_timesteps)
     mx, my, mz, mt = modes6
-    if width not in SUPPORTED_WIDTHS:
-        return False, f"width {width} not in {SUPPORTED_WIDTHS}"
+    if width not in SUPPORTED_WIDTHS + WIDE_WIDTHS:
+        return False, f"width {width} not in {SUPPORTED_WIDTHS} (nor in {WIDE_WIDTHS}, the round-2 widths)"
     if O > MAX_OUT:
         return False, f"out_channels = {O}: the fused projection head covers 1 <= out_channels <= {MAX_OUT}"
     if O > 1 and 2 * (2 * mz) > 128:
@@ -131,6 +135,9 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
     if O > 1 and width > 31:
         return False, (f"out_channels = {O} at width {width}: the multi-output head backward covers width <= 31 "
                        f"(its consumer registers run out at 32)")
+    if width in WIDE_WIDTHS and 2 * (2 * mz) > 128:
+        return False, (f"width {width} needs the round-2 route (2 * 2 * modes_z <= 128, here {4 * mz}); the round-1 "
+                       f"kernels cover widths {SUPPORTED_WIDTHS}")
     if P > 8:
         return False, "at most 8 peers (one NVSwitch box)"
     if Y % P or (2 * mz) % P:
@@ -861,11 +868,13 @@ class FusedDistributedFNO(nn.Module):
         return w3, w3t
 
     def _head_operators_cm(self):
-        """Operands of the channel-major head kernels: ``W3aug`` bf16 [H, 64] with column C = b3 (the hidden bias
-        rides through the MMA against the tile's row of ones) and ``W3^T`` as fp16 [ceil16(C+1), H]."""
+        """Operands of the channel-major head kernels: ``W3aug`` bf16 [H, 64] ([H, 128] at width 64) with column
+        C = b3 (the hidden bias rides through the MMA against the tile's row of ones) and ``W3^T`` as fp16
+        [ceil16(C+1), H]."""
         pl = self.plan
         W3, b3 = self._seg("linear3.W"), self._seg("linear3.b")
-        w3a = torch.zeros(pl.H, 64, device=self.device, dtype=torch.bfloat16)
+        # b3 in column C: one 64-column swizzle block up to width 63, two at width 64
+        w3a = torch.zeros(pl.H, 64 if pl.C + 1 <= 64 else 128, device=self.device, dtype=torch.bfloat16)
         w3a[:, :pl.C] = W3.to(torch.bfloat16)
         w3a[:, pl.C] = b3.to(torch.bfloat16)
         w3t = torch.zeros((pl.C + 1 + 15) // 16 * 16, pl.H, device=self.device, dtype=torch.float16)
