@@ -37,7 +37,8 @@ __device__ __forceinline__ float ldf<__nv_bfloat16>(const __nv_bfloat16* p) { re
 // One thread owns 8 consecutive z of one (b, x, y) -- a 16-byte bf16 vector of every output row it produces,
 // so a warp writes whole 256-byte z-lines -- and walks t and c.  Both GELUs run in packed fp16 (sm90_ptx.cuh):
 // the outer one is evaluated B*C*X*Y*Z*T times per step.  The few input values a thread needs stay in
-// registers when Tin == 1 (the benchmark / two-phase case) and are re-read through L1 otherwise (Cin <= 4, Tin <= 64).
+// registers when Tin == 1 (the benchmark / two-phase case) and are re-read through L1 otherwise (Cin <= 4, Tin <= 64;
+// more input channels run the one-warp-per-item kernels below).
 constexpr int kLiftMaxTin = 64;
 constexpr int kLiftMaxW = 4096;    // floats of shared memory for W1, b1 (+ packed W2, b2)
 
@@ -358,6 +359,361 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
 }
 
 // ------------------------------------------------------------------------------------------
+// lift, 5 <= Cin <= 16
+// ------------------------------------------------------------------------------------------
+// One warp owns one item (8 consecutive z of one (b, x, y)) and walks t.  Per t it runs in phases that map the lanes
+// differently, with a per-warp tile in shared memory between them:
+//   time lift : lane = (ci, z part of ZL = CINP / 4 values); a1 = gelu(b1 + W1 ._t x) in packed fp16 -> tile
+//   channels  : lane = output channel c (c + 32 for widths above 32); all CINP a1 values of the item come from the tile
+//   (backward) input side : lane = (ci, z part) again, reading the tile of dv = dh * gelu'(pre2) of every c.
+// So no thread ever holds CIN x 8 values.  With Tin > 1 the warp first copies the item's x (Cin runs of 8 * Tin
+// values, 5 KB at Cin = 16, Tin = 10 in fp32) into its own shared-memory slice with 16-byte loads; every t then reads
+// that copy, so x is read from global memory exactly once per call whatever T is.  (Tin == 1 keeps the lane's few x
+// values in registers instead.)  CINP (8 or 16) is the compile-time channel bound; W2 is zero-padded to it, so
+// channels ci >= Cin add exact zeros.
+constexpr int kLiftManyMaxC = 64;
+constexpr int kLiftManyWarps = 4;                      // warps per block (each with its own x slice)
+
+// elements between the shared-memory runs of two input channels: the run rounded up to 32 bytes, plus 16 bytes, so
+// that the lanes of different channels fall on different banks
+template <typename TIn>
+__host__ __device__ inline int lift_many_xs_stride(int Tin) {
+  const int words = 8 * Tin * static_cast<int>(sizeof(TIn)) / 4;
+  return ((words + 7) / 8 * 8 + 4) * 4 / static_cast<int>(sizeof(TIn));
+}
+
+// the warp's copy of one item's x: xs[ci * stride + z * Tin + ti] = x[b, ci, x, y, z0 + z, ti] (runs are 16-byte
+// multiples at 16-byte aligned addresses: Z % 8 == 0)
+template <typename TIn>
+__device__ __forceinline__ void lift_many_stage(const TIn* __restrict__ xb, long long xci_stride, int Cin, int Tin,
+                                                int lane, TIn* xs) {
+  const int nv = 8 * Tin * static_cast<int>(sizeof(TIn)) / 16;
+  const int sv = lift_many_xs_stride<TIn>(Tin) * static_cast<int>(sizeof(TIn)) / 16;
+  for (int j = lane; j < Cin * nv; j += 32) {
+    const int ci = j / nv, k = j - ci * nv;
+    reinterpret_cast<uint4*>(xs)[ci * sv + k] = reinterpret_cast<const uint4*>(xb + ci * xci_stride)[k];
+  }
+}
+
+template <int CINP>
+struct LiftManyLanes {
+  static constexpr int ZL = CINP / 4;                 // z values per lane in the input-side phases
+  static constexpr int kParts = 8 / ZL;               // lanes per input channel
+};
+
+template <typename TIn, int ZL>
+__device__ __forceinline__ void lift_many_load(const TIn* __restrict__ p, int stride, float (&v)[ZL]) {
+#pragma unroll
+  for (int z = 0; z < ZL; ++z) v[z] = ldf(p + z * stride);
+}
+
+// v[z] = b1[t] + sum_ti W1[t, ti] x[ci, z, ti] for this lane's ZL values of z
+template <typename TIn, int ZL, bool kRegs>
+__device__ __forceinline__ void lift_many_inner(const TIn* __restrict__ xz, const float (&xr)[ZL], int Tin,
+                                                const float* sW1t, float b1t, float (&v)[ZL]) {
+#pragma unroll
+  for (int z = 0; z < ZL; ++z) v[z] = kRegs ? fmaf(sW1t[0], xr[z], b1t) : b1t;
+  if (!kRegs) {
+    for (int ti = 0; ti < Tin; ++ti) {
+      float xv[ZL];
+      lift_many_load<TIn, ZL>(xz + ti, Tin, xv);
+      const float w = sW1t[ti];
+#pragma unroll
+      for (int z = 0; z < ZL; ++z) v[z] = fmaf(w, xv[z], v[z]);
+    }
+  }
+}
+
+template <typename TIn, int CINP, bool kRegs>
+__global__ void __launch_bounds__(32 * kLiftManyWarps)
+lift_fwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                     const float* __restrict__ W2, const float* __restrict__ b2, __nv_bfloat16* __restrict__ h,
+                     LiftDims d) {
+  using L = LiftManyLanes<CINP>;
+  constexpr int ZL = L::ZL, kWarps = kLiftManyWarps;
+  extern __shared__ uint4 fxs[];                                       // per warp: Cin runs of x (Tin > 1)
+  __shared__ float sw[kLiftMaxW];                                      // W1 [T][Tin], b1 [T]
+  __shared__ __half2 sW2[CINP * kLiftManyMaxC];                        // [CINP][C] (lanes = c: no bank conflicts)
+  __shared__ __half2 sb2[kLiftManyMaxC];
+  __shared__ __align__(16) __half2 sa1[kWarps][CINP][4];              // a1 of the warp's item at one t
+  float* sW1 = sw;
+  float* sb1 = sW1 + d.T * d.Tin;
+  for (int i = threadIdx.x; i < d.T * d.Tin; i += blockDim.x) sW1[i] = W1[i];
+  for (int i = threadIdx.x; i < d.T; i += blockDim.x) sb1[i] = b1[i];
+  for (int i = threadIdx.x; i < d.C * CINP; i += blockDim.x) {
+    const int c = i / CINP, ci = i % CINP;
+    sW2[ci * kLiftManyMaxC + c] = __float2half2_rn(ci < d.Cin ? W2[c * d.Cin + ci] : 0.f);  // zero beyond Cin
+  }
+  for (int i = threadIdx.x; i < d.C; i += blockDim.x) sb2[i] = __float2half2_rn(b2[i]);
+  __syncthreads();
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int ci = lane / L::kParts, zl = (lane % L::kParts) * ZL;        // input-side role
+  const bool live = ci < d.Cin;
+  const int zv = d.Z >> 3;
+  const long long plane = static_cast<long long>(d.X) * d.Y;
+  const long long nitems = static_cast<long long>(d.B) * plane * zv;
+  const long long hc_stride = plane * d.T * d.Z;
+  for (long long idx = blockIdx.x * static_cast<long long>(kWarps) + warp; idx < nitems;
+       idx += static_cast<long long>(gridDim.x) * kWarps) {              // warp-uniform
+    const int z0 = static_cast<int>(idx % zv) * 8;
+    const long long xy = (idx / zv) % plane;
+    const int b = static_cast<int>(idx / (zv * plane));
+    const TIn* xb = x + ((static_cast<long long>(b) * d.Cin * plane + xy) * d.Z + z0) * d.Tin;
+    const long long xci_stride = plane * d.Z * d.Tin;
+    const TIn* xz;
+    float xr[ZL];
+    if (kRegs) {
+      xz = xb + (live ? ci : 0) * xci_stride + zl;
+      if (live) lift_many_load<TIn, ZL>(xz, 1, xr);
+    } else {
+      const int xss = lift_many_xs_stride<TIn>(d.Tin);
+      TIn* xs = reinterpret_cast<TIn*>(fxs) + warp * d.Cin * xss;
+      lift_many_stage<TIn>(xb, xci_stride, d.Cin, d.Tin, lane, xs);   // the previous item's reads ended at __syncwarp
+      __syncwarp();
+      xz = xs + (live ? ci : 0) * xss + zl * d.Tin;
+    }
+    __nv_bfloat16* hb = h + ((static_cast<long long>(b) * d.C * plane + xy) * d.T) * d.Z + z0;
+    for (int t = 0; t < d.T; ++t) {
+      float v[ZL];
+      if (live) lift_many_inner<TIn, ZL, kRegs>(xz, xr, d.Tin, sW1 + t * d.Tin, sb1[t], v);
+#pragma unroll
+      for (int k = 0; k < ZL / 2; ++k)
+        sa1[warp][ci][zl / 2 + k] = live ? gelu_h2(h2_from_f32(v[2 * k], v[2 * k + 1])) : __float2half2_rn(0.f);
+      __syncwarp();
+      for (int c = lane; c < d.C; c += 32) {
+        __half2 acc[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) acc[k] = sb2[c];
+#pragma unroll
+        for (int j = 0; j < CINP; ++j) {
+          const uint4 a = *reinterpret_cast<const uint4*>(&sa1[warp][j][0]);
+          const __half2 w = sW2[j * kLiftManyMaxC + c];
+          acc[0] = __hfma2(w, h2_of_bits(a.x), acc[0]);
+          acc[1] = __hfma2(w, h2_of_bits(a.y), acc[1]);
+          acc[2] = __hfma2(w, h2_of_bits(a.z), acc[2]);
+          acc[3] = __hfma2(w, h2_of_bits(a.w), acc[3]);
+        }
+        uint32_t o[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) o[k] = h2_to_bf16x2(gelu_h2(acc[k]));
+        *reinterpret_cast<uint4*>(hb + c * hc_stride + static_cast<long long>(t) * d.Z) = make_uint4(o[0], o[1], o[2], o[3]);
+      }
+      __syncwarp();
+    }
+  }
+}
+
+// Backward of lift_fwd_many_kernel: the same outputs as lift_bwd_kernel.  Per t, after the time lift:
+//   channels   : lane c recomputes pre2 (packed fp16, as the forward), forms dv = dh * gelu'(pre2) in fp32, adds its
+//                db2[c] and dW2[c, :] = sum_z dv a1 partials to registers held over the whole loop (2 x CINP) and
+//                writes dv to the warp's [C][8] fp32 tile;
+//   input side : lane (ci, z part) forms da1 = W2^T dv from the tile (fp32 W2), e = da1 * gelu'(pre1), the time sums
+//                db1[t], dW1[t, :] (warp sums) and, with kDx, its own dx values: Tin == 1 keeps them in registers
+//                over t, otherwise the first t stores and later t add (read-modify-write of the lane's own values).
+// Everything the loss gradient multiplies is fp32; the GELU' evaluations are packed fp16.  W1 / b1 and their
+// gradient sums take dynamic shared memory (2 * (T * Tin + T) floats).
+template <typename TIn, int CINP, bool kRegs, bool kDx>
+__global__ void __launch_bounds__(32 * kLiftManyWarps, (CINP == 8 ? 4 : 3))        // 16 channels: more live values, no spills
+lift_bwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                     const float* __restrict__ W2, const float* __restrict__ b2,
+                     const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
+                     float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx) {
+  using L = LiftManyLanes<CINP>;
+  constexpr int ZL = L::ZL, kWarps = kLiftManyWarps, kU = kLiftManyMaxC / 32;
+  extern __shared__ float dsm[];                                       // W1, b1, their sums; then the x slices
+  __shared__ float sW2f[kLiftManyMaxC * CINP];                         // [C][CINP] fp32, zero beyond Cin
+  __shared__ __half2 sW2[CINP * kLiftManyMaxC];                        // the same, packed fp16, [CINP][C]
+  __shared__ __half2 sb2[kLiftManyMaxC];
+  __shared__ __align__(16) __half2 sa1[kWarps][CINP][4];
+  __shared__ __align__(16) float sdv[kWarps][kLiftManyMaxC][8];      // dv of the warp's item at one t
+  const int nw = d.T * d.Tin + d.T;
+  float* sW1 = dsm;
+  float* sb1 = sW1 + d.T * d.Tin;
+  float* gsW1 = dsm + nw;
+  float* gsb1 = gsW1 + d.T * d.Tin;
+  for (int i = threadIdx.x; i < nw; i += blockDim.x) { dsm[i] = i < d.T * d.Tin ? W1[i] : b1[i - d.T * d.Tin]; gsW1[i] = 0.f; }
+  for (int i = threadIdx.x; i < d.C * CINP; i += blockDim.x) {
+    const int c = i / CINP, ci = i % CINP;
+    sW2f[i] = ci < d.Cin ? W2[c * d.Cin + ci] : 0.f;
+    sW2[ci * kLiftManyMaxC + c] = __float2half2_rn(sW2f[i]);
+  }
+  for (int i = threadIdx.x; i < d.C; i += blockDim.x) sb2[i] = __float2half2_rn(b2[i]);
+  __syncthreads();
+
+  float accb2[kU], accW2[kU][CINP];
+#pragma unroll
+  for (int u = 0; u < kU; ++u) {
+    accb2[u] = 0.f;
+#pragma unroll
+    for (int j = 0; j < CINP; ++j) accW2[u][j] = 0.f;
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int ci = lane / L::kParts, zl = (lane % L::kParts) * ZL;
+  const bool live = ci < d.Cin;
+  const int zv = d.Z >> 3;
+  const long long plane = static_cast<long long>(d.X) * d.Y;
+  const long long nitems = static_cast<long long>(d.B) * plane * zv;
+  const long long hc_stride = plane * d.T * d.Z;
+  for (long long idx = blockIdx.x * static_cast<long long>(kWarps) + warp; idx < nitems;
+       idx += static_cast<long long>(gridDim.x) * kWarps) {              // warp-uniform
+    const int z0 = static_cast<int>(idx % zv) * 8;
+    const long long xy = (idx / zv) % plane;
+    const int b = static_cast<int>(idx / (zv * plane));
+    const long long xoff = ((((static_cast<long long>(b) * d.Cin) + (live ? ci : 0)) * plane + xy) * d.Z + z0 + zl) * d.Tin;
+    const TIn* xz;
+    float xr[ZL];
+    if (kRegs) {
+      xz = x + xoff;
+      if (live) lift_many_load<TIn, ZL>(xz, 1, xr);
+    } else {
+      const int xss = lift_many_xs_stride<TIn>(d.Tin);
+      TIn* xs = reinterpret_cast<TIn*>(dsm + (2 * nw + 3) / 4 * 4) + warp * d.Cin * xss;
+      __syncwarp();                                                    // the previous item's last reads of xs
+      lift_many_stage<TIn>(x + (xoff - (live ? ci : 0) * plane * d.Z * d.Tin - zl * d.Tin), plane * d.Z * d.Tin,
+                           d.Cin, d.Tin, lane, xs);
+      __syncwarp();
+      xz = xs + (live ? ci : 0) * xss + zl * d.Tin;
+    }
+    const __nv_bfloat16* gb = dh + ((static_cast<long long>(b) * d.C * plane + xy) * d.T) * d.Z + z0;
+    float dxr[ZL];
+#pragma unroll
+    for (int z = 0; z < ZL; ++z) dxr[z] = 0.f;
+    for (int t = 0; t < d.T; ++t) {
+      float g1[ZL];
+      {
+        float v[ZL];
+        if (live) lift_many_inner<TIn, ZL, kRegs>(xz, xr, d.Tin, sW1 + t * d.Tin, sb1[t], v);
+#pragma unroll
+        for (int k = 0; k < ZL / 2; ++k) {
+          GeluH2 vg;
+          vg.value = vg.grad = __float2half2_rn(0.f);
+          if (live) vg = gelu_vg_h2(h2_from_f32(v[2 * k], v[2 * k + 1]));
+          sa1[warp][ci][zl / 2 + k] = vg.value;
+          const float2 gv = __half22float2(vg.grad);
+          g1[2 * k] = gv.x; g1[2 * k + 1] = gv.y;
+        }
+      }
+      __syncwarp();
+#pragma unroll
+      for (int u = 0; u < kU; ++u) {
+        const int c = lane + 32 * u;
+        if (c < d.C) {
+          const uint4 gw = *reinterpret_cast<const uint4*>(gb + c * hc_stride + static_cast<long long>(t) * d.Z);
+          __half2 acc[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) acc[k] = sb2[c];
+#pragma unroll
+          for (int j = 0; j < CINP; ++j) {
+            const uint4 a = *reinterpret_cast<const uint4*>(&sa1[warp][j][0]);
+            const __half2 w = sW2[j * kLiftManyMaxC + c];
+            acc[0] = __hfma2(w, h2_of_bits(a.x), acc[0]);
+            acc[1] = __hfma2(w, h2_of_bits(a.y), acc[1]);
+            acc[2] = __hfma2(w, h2_of_bits(a.z), acc[2]);
+            acc[3] = __hfma2(w, h2_of_bits(a.w), acc[3]);
+          }
+          const uint32_t gws[4] = {gw.x, gw.y, gw.z, gw.w};
+          float dv[8];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const float2 gr = __half22float2(gelu_vg_h2(acc[k]).grad);
+            const float2 g = unpack_bf16x2(gws[k]);
+            dv[2 * k] = g.x * gr.x; dv[2 * k + 1] = g.y * gr.y;
+          }
+          float sb = 0.f;
+#pragma unroll
+          for (int z = 0; z < 8; ++z) sb += dv[z];
+          accb2[u] += sb;
+#pragma unroll
+          for (int j = 0; j < CINP; ++j) {
+            const uint4 a = *reinterpret_cast<const uint4*>(&sa1[warp][j][0]);
+            const uint32_t aw[4] = {a.x, a.y, a.z, a.w};
+            float s = 0.f;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const float2 af = __half22float2(h2_of_bits(aw[k]));
+              s = fmaf(dv[2 * k], af.x, s);
+              s = fmaf(dv[2 * k + 1], af.y, s);
+            }
+            accW2[u][j] += s;
+          }
+          float4* dst = reinterpret_cast<float4*>(&sdv[warp][c][0]);
+          dst[0] = make_float4(dv[0], dv[1], dv[2], dv[3]);
+          dst[1] = make_float4(dv[4], dv[5], dv[6], dv[7]);
+        }
+      }
+      __syncwarp();
+      float e[ZL];
+#pragma unroll
+      for (int z = 0; z < ZL; ++z) e[z] = 0.f;
+      if (live) {
+        for (int c = 0; c < d.C; ++c) {
+          const float w = sW2f[c * CINP + ci];
+#pragma unroll
+          for (int z = 0; z < ZL; ++z) e[z] = fmaf(w, sdv[warp][c][zl + z], e[z]);
+        }
+      }
+      float sb1v = 0.f;
+#pragma unroll
+      for (int z = 0; z < ZL; ++z) { e[z] *= g1[z]; sb1v += e[z]; }
+      sb1v = warp_sum(sb1v);
+      if (lane == 0) atomicAdd(&gsb1[t], sb1v);
+      if (kRegs) {
+        float s = 0.f;
+#pragma unroll
+        for (int z = 0; z < ZL; ++z) s = fmaf(e[z], live ? xr[z] : 0.f, s);
+        s = warp_sum(s);
+        if (lane == 0) atomicAdd(&gsW1[t], s);
+        if (kDx) {
+          const float w = sW1[t];
+#pragma unroll
+          for (int z = 0; z < ZL; ++z) dxr[z] = fmaf(w, e[z], dxr[z]);
+        }
+      } else {
+        for (int ti = 0; ti < d.Tin; ++ti) {
+          float xv[ZL];
+          if (live) lift_many_load<TIn, ZL>(xz + ti, d.Tin, xv);
+          float s = 0.f;
+#pragma unroll
+          for (int z = 0; z < ZL; ++z) s = fmaf(e[z], live ? xv[z] : 0.f, s);
+          s = warp_sum(s);
+          if (lane == 0) atomicAdd(&gsW1[t * d.Tin + ti], s);
+          if (kDx && live) {
+            const float w = sW1[t * d.Tin + ti];
+            float* p = dx + xoff + ti;
+#pragma unroll
+            for (int z = 0; z < ZL; ++z) p[z * d.Tin] = t == 0 ? w * e[z] : fmaf(w, e[z], p[z * d.Tin]);
+          }
+        }
+      }
+    }
+    if (kDx && kRegs && live) {
+#pragma unroll
+      for (int z = 0; z < ZL; z += 2) *reinterpret_cast<float2*>(dx + xoff + z) = make_float2(dxr[z], dxr[z + 1]);
+    }
+  }
+  // channel sums: lane c holds the partials of channels c and c + 32 (no two lanes of a warp share a channel)
+  __syncthreads();
+  float* gsW2 = &sdv[0][0][0];                                         // [C][CINP] + [C], the dv tiles are done
+  for (int i = threadIdx.x; i < d.C * CINP + d.C; i += blockDim.x) gsW2[i] = 0.f;
+  __syncthreads();
+#pragma unroll
+  for (int u = 0; u < kU; ++u) {
+    const int c = lane + 32 * u;
+    if (c < d.C) {
+      atomicAdd(&gsW2[d.C * CINP + c], accb2[u]);
+#pragma unroll
+      for (int j = 0; j < CINP; ++j) atomicAdd(&gsW2[c * CINP + j], accW2[u][j]);
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < d.T * d.Tin; i += blockDim.x) atomicAdd(&gW1[i], gsW1[i]);
+  for (int i = threadIdx.x; i < d.T; i += blockDim.x) atomicAdd(&gb1[i], gsb1[i]);
+  for (int i = threadIdx.x; i < d.C * d.Cin; i += blockDim.x) atomicAdd(&gW2[i], gsW2[(i / d.Cin) * CINP + i % d.Cin]);
+  for (int i = threadIdx.x; i < d.C; i += blockDim.x) atomicAdd(&gb2[i], gsW2[d.C * CINP + i]);
+}
+
+// ------------------------------------------------------------------------------------------
 // bypass conv + GELU
 // ------------------------------------------------------------------------------------------
 // Each thread owns 2 consecutive z of one (b, x, y, t) and all C channels.
@@ -613,16 +969,106 @@ const char* gelu_probe(const float* x, float* y, float* dy, long long n, cudaStr
 
 static const char* lift_check(const LiftDims& d) {
   if (d.Z % 8) return "lift: Z must be a multiple of 8";
-  if (d.Cin < 1 || d.Cin > 4) return "lift: supported input channel counts are 1..4";
+  if (d.Cin < 1 || d.Cin > 16) return "lift: supported input channel counts are 1..16";
   if (d.Tin < 1 || d.Tin > kLiftMaxTin) return "lift: 1 <= Tin <= 64";
   if (d.C > 64) return "lift: C <= 64";
   if (d.T * d.Tin + d.T + 2 * (d.C * d.Cin + d.C) > kLiftMaxW) return "lift: weights exceed shared memory budget";
   return nullptr;
 }
 
+// 5 <= Cin <= 16: one warp per item (lift_fwd_many_kernel), channels padded to 8 or 16
+// bytes of the per-warp x slices of one block (Tin > 1; up to 129 KB at Cin = 16, Tin = 64 in fp32)
+template <typename TIn>
+static size_t lift_many_xs_bytes(int Cin, int Tin) {
+  return Tin == 1 ? 0 : static_cast<size_t>(kLiftManyWarps) * Cin * lift_many_xs_stride<TIn>(Tin) * sizeof(TIn);
+}
+
+// opts a kernel into the largest dynamic shared memory its launches ask for (once per instantiation)
+template <typename K>
+static const char* lift_many_allow_smem(K kern, bool& done, size_t bytes) {
+  if (done) return nullptr;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+  if (e != cudaSuccess) return cudaGetErrorString(e);
+  done = true;
+  return nullptr;
+}
+
+template <typename TIn, int CINP, bool kRegs>
+static const char* lift_fwd_many_launch(const void* x, const float* W1, const float* b1, const float* W2,
+                                        const float* b2, void* h, LiftDims d, int grid, cudaStream_t s) {
+  auto kern = lift_fwd_many_kernel<TIn, CINP, kRegs>;
+  static bool attr = false;
+  if (const char* e = lift_many_allow_smem(kern, attr, lift_many_xs_bytes<TIn>(16, kLiftMaxTin))) return e;
+  kern<<<grid, 32 * kLiftManyWarps, lift_many_xs_bytes<TIn>(d.Cin, d.Tin), s>>>(
+      static_cast<const TIn*>(x), W1, b1, W2, b2, static_cast<__nv_bfloat16*>(h), d);
+  return nullptr;
+}
+
+static const char* lift_fwd_many(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
+                                 const float* b2, void* h, LiftDims d, int num_sms, cudaStream_t s) {
+  const long long nitems = static_cast<long long>(d.B) * d.X * d.Y * (d.Z / 8);
+  const int grid = grid_for(32 * nitems, 32 * kLiftManyWarps, num_sms, 8);
+  const bool regs = d.Tin == 1;
+#define DFNO_LIFT_FWD_MANY(T_, CINP_)                                                          \
+  (regs ? lift_fwd_many_launch<T_, CINP_, true>(x, W1, b1, W2, b2, h, d, grid, s)               \
+        : lift_fwd_many_launch<T_, CINP_, false>(x, W1, b1, W2, b2, h, d, grid, s))
+  const char* err;
+  if (x_is_bf16)
+    err = d.Cin <= 8 ? DFNO_LIFT_FWD_MANY(__nv_bfloat16, 8) : DFNO_LIFT_FWD_MANY(__nv_bfloat16, 16);
+  else
+    err = d.Cin <= 8 ? DFNO_LIFT_FWD_MANY(float, 8) : DFNO_LIFT_FWD_MANY(float, 16);
+#undef DFNO_LIFT_FWD_MANY
+  if (err) return err;
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
+template <typename TIn, int CINP, bool kRegs, bool kDx>
+static const char* lift_bwd_many_launch(const void* x, const float* W1, const float* b1, const float* W2,
+                                        const float* b2, const void* dh, float* gW1, float* gb1, float* gW2,
+                                        float* gb2, float* dx, LiftDims d, int grid, cudaStream_t s) {
+  auto kern = lift_bwd_many_kernel<TIn, CINP, kRegs, kDx>;
+  static bool attr = false;                     // W1, b1 and their sums (up to 2 * kLiftMaxW floats), then x slices
+  if (const char* e = lift_many_allow_smem(kern, attr, 2 * kLiftMaxW * sizeof(float) +
+                                                           lift_many_xs_bytes<TIn>(16, kLiftMaxTin)))
+    return e;
+  const size_t smem = (2 * static_cast<size_t>(d.T * d.Tin + d.T) + 3) / 4 * 4 * sizeof(float) +
+                      lift_many_xs_bytes<TIn>(d.Cin, d.Tin);
+  kern<<<grid, 32 * kLiftManyWarps, smem, s>>>(static_cast<const TIn*>(x), W1, b1, W2, b2, static_cast<const __nv_bfloat16*>(dh), gW1,
+                               gb1, gW2, gb2, d, dx);
+  return nullptr;
+}
+
+// 5 <= Cin <= 16: one warp per item (lift_bwd_many_kernel)
+static const char* lift_bwd_many(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
+                                 const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2,
+                                 float* dx, LiftDims d, int num_sms, cudaStream_t s) {
+  const long long nitems = static_cast<long long>(d.B) * d.X * d.Y * (d.Z / 8);
+  const int grid = grid_for(32 * nitems, 32 * kLiftManyWarps, num_sms, 8);
+  const bool regs = d.Tin == 1;
+#define DFNO_LIFT_BWD_MANY3(T_, CINP_, R_, DX_) \
+  lift_bwd_many_launch<T_, CINP_, R_, DX_>(x, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, grid, s)
+#define DFNO_LIFT_BWD_MANY2(T_, CINP_, R_) \
+  (dx ? DFNO_LIFT_BWD_MANY3(T_, CINP_, R_, true) : DFNO_LIFT_BWD_MANY3(T_, CINP_, R_, false))
+#define DFNO_LIFT_BWD_MANY1(T_, CINP_) \
+  (regs ? DFNO_LIFT_BWD_MANY2(T_, CINP_, true) : DFNO_LIFT_BWD_MANY2(T_, CINP_, false))
+  const char* err;
+  if (x_is_bf16)
+    err = d.Cin <= 8 ? DFNO_LIFT_BWD_MANY1(__nv_bfloat16, 8) : DFNO_LIFT_BWD_MANY1(__nv_bfloat16, 16);
+  else
+    err = d.Cin <= 8 ? DFNO_LIFT_BWD_MANY1(float, 8) : DFNO_LIFT_BWD_MANY1(float, 16);
+#undef DFNO_LIFT_BWD_MANY1
+#undef DFNO_LIFT_BWD_MANY2
+#undef DFNO_LIFT_BWD_MANY3
+  if (err) return err;
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
 const char* lift_fwd(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
                      const float* b2, void* h, LiftDims d, int num_sms, cudaStream_t s) {
   if (const char* e = lift_check(d)) return e;
+  if (d.Cin > 4) return lift_fwd_many(x, x_is_bf16, W1, b1, W2, b2, h, d, num_sms, s);
   const long long nitems = static_cast<long long>(d.B) * d.X * d.Y * (d.Z / 8);
   const int grid = grid_for(nitems, 256, num_sms, 4);
   const bool regs = d.Tin == 1;
@@ -693,6 +1139,7 @@ const char* lift_bwd(const void* x, int x_is_bf16, const float* W1, const float*
                      LiftDims d, int num_sms, cudaStream_t s) {
   if (const char* e = lift_check(d)) return e;
   if (dx && reinterpret_cast<uintptr_t>(dx) % 8) return "lift_bwd: dx must be 8-byte aligned";
+  if (d.Cin > 4) return lift_bwd_many(x, x_is_bf16, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, num_sms, s);
   const long long nitems = static_cast<long long>(d.B) * d.X * d.Y * (d.Z / 8);
   const int split = d.C > 32 ? 8 : 4;                                 // lanes per item (see lift_bwd_kernel)
   const int grid = grid_for(split * nitems, 128, num_sms, 4);

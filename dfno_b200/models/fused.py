@@ -50,6 +50,7 @@ SUPPORTED_WIDTHS = (4, 8, 12, 16, 20, 24, 32)
 # mix, lift backward and channel-major head kernels exist for them, the round-1 kernels do not
 WIDE_WIDTHS = (48, 64)
 MAX_OUT = 4                  # output channels of the multi-output head kernels (csrc/head_multi_sm90.cu)
+MAX_IN = 16                  # input channels of the lift kernels (Cin > 4: lift_*_many_kernel, csrc/pointwise.cu)
 MAX_N = 256                  # n_pad limit of dft_gemm (accumulator columns of one 64-row warpgroup tile)
 HBM_BUDGET = 72 * 2 ** 30    # of an H100's 80 GB: leave room for the CUDA context, NCCL and the allocator
 HEAD_HIDDEN = 128
@@ -142,8 +143,8 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
         return False, "at most 8 peers (one NVSwitch box)"
     if Y % P or (2 * mz) % P:
         return False, "Y and 2*modes_z must divide evenly over the pencil"
-    if Cin > 4 or Tin > 64:
-        return False, "lift kernel covers Cin <= 4 and Tin <= 64"
+    if Cin > MAX_IN or Tin > 64:
+        return False, f"lift kernels cover Cin <= {MAX_IN} and Tin <= 64"
     lift_w = T * Tin + T + 2 * (width * Cin + width)
     if lift_w > LIFT_MAX_W:
         return False, (f"lift weights need {lift_w} floats of shared memory, more than the lift kernel's "
@@ -431,6 +432,7 @@ class EnginePlan:
         legacy = not self.fused_pw
         P = self.world
         act, cl = self.n_act * bf, self.npos * self.CP * bf
+        x_in = self.B * self.S // self.T * self.Cin * self.Tin * f32    # the network input (fp32, as memory_bytes)
         Z1, S1, S2, S3, T2, U = (self.n_Z1 * bf, self.n_S1 * bf, self.n_S2 * bf, self.n_S3 * bf, self.n_T2 * bf,
                                  self.n_U * bf)
         T1 = self.n_T1 // self.mtp * self.mt * bf                      # valid (kt < mt) part
@@ -448,7 +450,7 @@ class EnginePlan:
             chain += [("permS1", 2 * S1, 0), ("permT1", 2 * T1, 0)]
         st = [(n, 2 * nb, b, l) for n, b, l in chain]                  # forward + adjoint chain per block
         st += [("spectral_mix fwd", nb, 2 * S3 + W, 0), ("spectral_mix bwd", nb, 3 * S3 + 2 * W, 0),
-               ("lift fwd", 1, act, 0), ("lift bwd", 1, act, 0), ("adam", 1, 7 * self.n_theta * f32, 0)]
+               ("lift fwd", 1, act + x_in, 0), ("lift bwd", 1, act + x_in, 0), ("adam", 1, 7 * self.n_theta * f32, 0)]
         if legacy:
             st += [("iG1a add (bwd)", nb, act, 0), ("bypass fwd", nb, 4 * act, 0), ("bypass bwd", nb, 5 * act, 0),
                    ("head fwd", 1, cl + self.O * self.npos * f32, 0), ("head bwd", 1, 2 * cl + self.O * self.npos * f32, 0)]
