@@ -77,5 +77,54 @@ int set_rowmap(RowMap* mp, int nrl, const int* R, const long long* SR) {
   return 0;
 }
 
+// Row map of a zero-padded activation (the padded-layout head kernels): up to 5 digits (b, x, y, t, z can all be
+// separate), each with the extent of its interior; a row with any digit at or beyond its bound lies in the pad region
+// and has no output element.
+constexpr int kPadDigits = 5;
+struct PadRowMap {
+  int nrl;
+  int R[kPadDigits], lim[kPadDigits];
+  long long SR[kPadDigits];
+  unsigned long long Rm[kPadDigits];
+  int Rs[kPadDigits];
+};
+
+// element offset of row r in the public output, or -1 for a pad row
+__device__ __forceinline__ long long pad_row_to_offset(const PadRowMap& e, uint32_t r) {
+  long long off = 0;
+  bool inside = true;
+#pragma unroll
+  for (int l = 0; l < kPadDigits; ++l) {
+    if (l < e.nrl) {
+      uint32_t d = r;
+      if (l != e.nrl - 1) {
+        const uint32_t q = static_cast<uint32_t>((static_cast<unsigned long long>(r) * e.Rm[l]) >> e.Rs[l]);
+        d = r - q * static_cast<uint32_t>(e.R[l]);
+        r = q;
+      }
+      inside = inside && d < static_cast<uint32_t>(e.lim[l]);
+      off += static_cast<long long>(d) * e.SR[l];
+    }
+  }
+  return inside ? off : -1;
+}
+
+int set_padrowmap(PadRowMap* mp, int nrl, const int* R, const long long* SR, const int* lim) {
+  if (nrl < 1 || nrl > kPadDigits) return -1;
+  mp->nrl = nrl;
+  for (int i = 0; i < kPadDigits; ++i) {
+    mp->R[i] = i < nrl ? R[i] : 1;
+    mp->SR[i] = i < nrl ? SR[i] : 0;
+    mp->lim[i] = i < nrl ? lim[i] : 1;
+    if (mp->lim[i] > mp->R[i]) return -1;
+    const unsigned d = static_cast<unsigned>(mp->R[i] > 0 ? mp->R[i] : 1);      // as fill_magic
+    int s = 0;
+    while ((1ull << s) < d) ++s;
+    mp->Rm[i] = ((1ull << (31 + s)) / d) + 1;
+    mp->Rs[i] = 31 + s;
+  }
+  return 0;
+}
+
 }  // namespace
 }  // namespace dfno

@@ -42,11 +42,10 @@ struct HeadMultiFwdParams {
   RowMap map;
 };
 
-// KR: channels + the ones row, padded to 16 (the K of the MMA); O: output channels
-template <int KR, int O>
-__global__ void __launch_bounds__(kThreadsMF, 1)
-head_fwd_multi_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
-                      const HeadMultiFwdParams p) {
+// KR: channels + the ones row, padded to 16 (the K of the MMA); O: output channels.  kPad: as head_fwd_kernel.
+template <int KR, int O, bool kPad>
+__device__ __forceinline__ void head_fwd_multi_body(const CUtensorMap& tmH, const CUtensorMap& tmW3,
+                                                    const HeadMultiFwdParams p, const PadRowMap pm) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* s_w3 = smem;                                    // [128 hid][64] K-major, column C = b3
   uint8_t* s_a = smem + 16384;                             // stages x 2 halves x [KR rows][64 pos]
@@ -134,7 +133,9 @@ head_fwd_multi_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_cons
 #pragma unroll
       for (int j = 0; j < 16; ++j) gh[k][j] = h2_bits(gelu_h2(h2_from_f32(a[4 * j], a[4 * j + 1])));
     }
-    const long long base = pos < p.S ? row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos)) : 0;
+    long long base;
+    if constexpr (kPad) base = pos < p.S ? pad_row_to_offset(pm, static_cast<uint32_t>(b * p.S + pos)) : -1;
+    else base = pos < p.S ? row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos)) : 0;
 #pragma unroll
     for (int o = 0; o < O; ++o) {
       uint32_t w4[16];
@@ -159,9 +160,23 @@ head_fwd_multi_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_cons
         sum += __shfl_xor_sync(0xffffffffu, sum, 2);
         out[k] = sum;
       }
-      if (pos < p.S) p.out[base + o * p.plane] = s_b4[o] + pick4(out, cq);
+      if (kPad ? base >= 0 : pos < p.S) p.out[base + o * p.plane] = s_b4[o] + pick4(out, cq);
     }
   }
+}
+
+template <int KR, int O>
+__global__ void __launch_bounds__(kThreadsMF, 1)
+head_fwd_multi_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
+                      const HeadMultiFwdParams p) {
+  head_fwd_multi_body<KR, O, false>(tmH, tmW3, p, PadRowMap{});
+}
+
+template <int KR, int O>
+__global__ void __launch_bounds__(kThreadsMF, 1)
+head_fwd_multi_pad_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
+                          const HeadMultiFwdParams p, const __grid_constant__ PadRowMap pm) {
+  head_fwd_multi_body<KR, O, true>(tmH, tmW3, p, pm);
 }
 
 // ================================================================================ backward
@@ -186,12 +201,12 @@ struct HeadMultiBwdParams {
 // One consumer warpgroup per tile of 128 positions, as head_bwd2_kernel.  Per 64-unit hidden half, epilogue A turns
 // the MMA1 accumulator into P' (register A operand of MMA2, stored with stmatrix for MMA3) and G (stored with stmatrix
 // for MMA4); epilogue B stages g as bf16 [C][128 positions] with stmatrix.trans for two TMA stores.
-// KR: channels + the ones row, padded to 16 (the N of MMA2 / MMA3 and the accumulator width); O: output channels
-template <int KR, int O>
-__global__ void __launch_bounds__(kThreadsMB, 1)
-head_bwd_multi_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
-                      const __grid_constant__ CUtensorMap tmW3T, const __grid_constant__ CUtensorMap tmG,
-                      const HeadMultiBwdParams p) {
+// KR: channels + the ones row, padded to 16 (the N of MMA2 / MMA3 and the accumulator width); O: output channels.
+// kPad: as head_bwd2_kernel (pad rows read dout as 0).
+template <int KR, int O, bool kPad>
+__device__ __forceinline__ void head_bwd_multi_body(const CUtensorMap& tmH, const CUtensorMap& tmW3,
+                                                    const CUtensorMap& tmW3T, const CUtensorMap& tmG,
+                                                    const HeadMultiBwdParams p, const PadRowMap pm) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr uint32_t half_bytes = KR * 128;
   constexpr uint32_t tile_bytes = 2 * half_bytes;
@@ -324,11 +339,13 @@ head_bwd_multi_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_cons
     const int b = static_cast<int>(tile / p.tiles_per_b);
     const long long p0 = (tile % p.tiles_per_b) * 128;
     const long long pos = p0 + my_row;
-    const long long base = pos < p.S ? row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos)) : 0;
+    long long base;
+    if constexpr (kPad) base = pos < p.S ? pad_row_to_offset(pm, static_cast<uint32_t>(b * p.S + pos)) : -1;
+    else base = pos < p.S ? row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos)) : 0;
     __half2 dsh[O][2];                               // s dout[row, o] of the thread's rows frag_row(q, lane, 2m + {0, 1})
 #pragma unroll
     for (int o = 0; o < O; ++o) {
-      const float dl = pos < p.S ? p.dout[base + o * p.plane] : 0.f;
+      const float dl = (kPad ? base >= 0 : pos < p.S) ? p.dout[base + o * p.plane] : 0.f;
       float sum = dl;                                // db4: this warp's 32 rows, one shared-memory add per warp
 #pragma unroll
       for (int m = 16; m > 0; m >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, m);
@@ -479,48 +496,74 @@ head_bwd_multi_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_cons
   }
 }
 
+template <int KR, int O>
+__global__ void __launch_bounds__(kThreadsMB, 1)
+head_bwd_multi_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
+                      const __grid_constant__ CUtensorMap tmW3T, const __grid_constant__ CUtensorMap tmG,
+                      const HeadMultiBwdParams p) {
+  head_bwd_multi_body<KR, O, false>(tmH, tmW3, tmW3T, tmG, p, PadRowMap{});
+}
+
+template <int KR, int O>
+__global__ void __launch_bounds__(kThreadsMB, 1)
+head_bwd_multi_pad_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
+                          const __grid_constant__ CUtensorMap tmW3T, const __grid_constant__ CUtensorMap tmG,
+                          const HeadMultiBwdParams p, const __grid_constant__ PadRowMap pm) {
+  head_bwd_multi_body<KR, O, true>(tmH, tmW3, tmW3T, tmG, p, pm);
+}
+
 // ================================================================================ dispatch over (KR, O)
-template <int KR, int O>
+template <int KR, int O, bool kPad>
 void launch_fwd(int grid, uint32_t smem, cudaStream_t st, const CUtensorMap& a, const CUtensorMap& b,
-                const HeadMultiFwdParams& p) {
-  head_fwd_multi_kernel<KR, O><<<grid, kThreadsMF, smem, st>>>(a, b, p);
+                const HeadMultiFwdParams p, const PadRowMap pm) {
+  if constexpr (kPad) head_fwd_multi_pad_kernel<KR, O><<<grid, kThreadsMF, smem, st>>>(a, b, p, pm);
+  else head_fwd_multi_kernel<KR, O><<<grid, kThreadsMF, smem, st>>>(a, b, p);
 }
-template <int KR, int O>
+template <int KR, int O, bool kPad>
 void launch_bwd(int grid, uint32_t smem, cudaStream_t st, const CUtensorMap& a, const CUtensorMap& b,
-                const CUtensorMap& c, const CUtensorMap& d, const HeadMultiBwdParams& p) {
-  head_bwd_multi_kernel<KR, O><<<grid, kThreadsMB, smem, st>>>(a, b, c, d, p);
+                const CUtensorMap& c, const CUtensorMap& d, const HeadMultiBwdParams p, const PadRowMap pm) {
+  if constexpr (kPad) head_bwd_multi_pad_kernel<KR, O><<<grid, kThreadsMB, smem, st>>>(a, b, c, d, p, pm);
+  else head_bwd_multi_kernel<KR, O><<<grid, kThreadsMB, smem, st>>>(a, b, c, d, p);
 }
 
-template <int KR>
+template <int KR, bool kPad>
 const void* fwd_fn(int O) {
-  return O == 1 ? reinterpret_cast<const void*>(head_fwd_multi_kernel<KR, 1>)
-       : O == 2 ? reinterpret_cast<const void*>(head_fwd_multi_kernel<KR, 2>)
-       : O == 3 ? reinterpret_cast<const void*>(head_fwd_multi_kernel<KR, 3>)
-                : reinterpret_cast<const void*>(head_fwd_multi_kernel<KR, 4>);
+  return O == 1 ? (kPad ? reinterpret_cast<const void*>(head_fwd_multi_pad_kernel<KR, 1>)
+                      : reinterpret_cast<const void*>(head_fwd_multi_kernel<KR, 1>))
+       : O == 2 ? (kPad ? reinterpret_cast<const void*>(head_fwd_multi_pad_kernel<KR, 2>)
+                      : reinterpret_cast<const void*>(head_fwd_multi_kernel<KR, 2>))
+       : O == 3 ? (kPad ? reinterpret_cast<const void*>(head_fwd_multi_pad_kernel<KR, 3>)
+                      : reinterpret_cast<const void*>(head_fwd_multi_kernel<KR, 3>))
+                : (kPad ? reinterpret_cast<const void*>(head_fwd_multi_pad_kernel<KR, 4>)
+                      : reinterpret_cast<const void*>(head_fwd_multi_kernel<KR, 4>));
 }
-template <int KR>
+template <int KR, bool kPad>
 const void* bwd_fn(int O) {
-  return O == 1 ? reinterpret_cast<const void*>(head_bwd_multi_kernel<KR, 1>)
-       : O == 2 ? reinterpret_cast<const void*>(head_bwd_multi_kernel<KR, 2>)
-       : O == 3 ? reinterpret_cast<const void*>(head_bwd_multi_kernel<KR, 3>)
-                : reinterpret_cast<const void*>(head_bwd_multi_kernel<KR, 4>);
+  return O == 1 ? (kPad ? reinterpret_cast<const void*>(head_bwd_multi_pad_kernel<KR, 1>)
+                      : reinterpret_cast<const void*>(head_bwd_multi_kernel<KR, 1>))
+       : O == 2 ? (kPad ? reinterpret_cast<const void*>(head_bwd_multi_pad_kernel<KR, 2>)
+                      : reinterpret_cast<const void*>(head_bwd_multi_kernel<KR, 2>))
+       : O == 3 ? (kPad ? reinterpret_cast<const void*>(head_bwd_multi_pad_kernel<KR, 3>)
+                      : reinterpret_cast<const void*>(head_bwd_multi_kernel<KR, 3>))
+                : (kPad ? reinterpret_cast<const void*>(head_bwd_multi_pad_kernel<KR, 4>)
+                      : reinterpret_cast<const void*>(head_bwd_multi_kernel<KR, 4>));
 }
 
-template <int KR>
+template <int KR, bool kPad>
 void launch_fwd_o(int O, int grid, uint32_t smem, cudaStream_t st, const CUtensorMap& a, const CUtensorMap& b,
-                  const HeadMultiFwdParams& p) {
-  if (O == 1) launch_fwd<KR, 1>(grid, smem, st, a, b, p);
-  else if (O == 2) launch_fwd<KR, 2>(grid, smem, st, a, b, p);
-  else if (O == 3) launch_fwd<KR, 3>(grid, smem, st, a, b, p);
-  else launch_fwd<KR, 4>(grid, smem, st, a, b, p);
+                  const HeadMultiFwdParams p, const PadRowMap pm) {
+  if (O == 1) launch_fwd<KR, 1, kPad>(grid, smem, st, a, b, p, pm);
+  else if (O == 2) launch_fwd<KR, 2, kPad>(grid, smem, st, a, b, p, pm);
+  else if (O == 3) launch_fwd<KR, 3, kPad>(grid, smem, st, a, b, p, pm);
+  else launch_fwd<KR, 4, kPad>(grid, smem, st, a, b, p, pm);
 }
-template <int KR>
+template <int KR, bool kPad>
 void launch_bwd_o(int O, int grid, uint32_t smem, cudaStream_t st, const CUtensorMap& a, const CUtensorMap& b,
-                  const CUtensorMap& c, const CUtensorMap& d, const HeadMultiBwdParams& p) {
-  if (O == 1) launch_bwd<KR, 1>(grid, smem, st, a, b, c, d, p);
-  else if (O == 2) launch_bwd<KR, 2>(grid, smem, st, a, b, c, d, p);
-  else if (O == 3) launch_bwd<KR, 3>(grid, smem, st, a, b, c, d, p);
-  else launch_bwd<KR, 4>(grid, smem, st, a, b, c, d, p);
+                  const CUtensorMap& c, const CUtensorMap& d, const HeadMultiBwdParams p, const PadRowMap pm) {
+  if (O == 1) launch_bwd<KR, 1, kPad>(grid, smem, st, a, b, c, d, p, pm);
+  else if (O == 2) launch_bwd<KR, 2, kPad>(grid, smem, st, a, b, c, d, p, pm);
+  else if (O == 3) launch_bwd<KR, 3, kPad>(grid, smem, st, a, b, c, d, p, pm);
+  else launch_bwd<KR, 4, kPad>(grid, smem, st, a, b, c, d, p, pm);
 }
 
 const char* set_max_smem(const void* fn, bool* done) {
@@ -536,8 +579,8 @@ const char* set_max_smem(const void* fn, bool* done) {
 // h: bf16 [B*C, S] channel-major; W3aug: bf16 [128, 64] with column C = b3; w4b4: fp32 [O*128 + O] (W4 [O, 128] then
 // b4 [O]); out: fp32, row addressed through the row digits (row = b*S + position), output channel o at + o*plane.
 const char* head_fwd_multi(const void* h, const void* W3aug, const float* w4b4, float* out, int B, int C, long long S,
-                           int O, long long plane, int nrl, const int* R, const long long* SR, int num_sms,
-                           cudaStream_t stream) {
+                           int O, long long plane, int nrl, const int* R, const long long* SR, const int* lim,
+                           int num_sms, cudaStream_t stream) {
   if (C < 1 || C > 47) return "head_fwd_multi: 1 <= C <= 47";
   if (O < 1 || O > kMaxOut) return "head_fwd_multi: 1 <= O <= 4";
   if (S % 8 || S > (1ll << 31) - 256 || static_cast<long long>(B) * S > (1ll << 31) - 256)
@@ -545,20 +588,27 @@ const char* head_fwd_multi(const void* h, const void* W3aug, const float* w4b4, 
   HeadMultiFwdParams p{};
   p.B = B; p.C = C; p.S = S; p.tiles_per_b = (S + 127) / 128; p.plane = plane;
   p.w4b4 = w4b4; p.out = out;
-  if (set_rowmap(&p.map, nrl, R, SR)) return "head_fwd_multi: 1..4 row digits";
+  PadRowMap pm{};
+  if (lim ? set_padrowmap(&pm, nrl, R, SR, lim) : set_rowmap(&p.map, nrl, R, SR))
+    return lim ? "head_fwd_multi: 1..5 row digits, each bound within its radix" : "head_fwd_multi: 1..4 row digits";
   CUtensorMap tmH, tmW3;
   if (make_map_2d(&tmH, h, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (h) failed";
   if (make_map_2d(&tmW3, W3aug, 64, 128, 64, 64, 128)) return "tensor map (W3) failed";
   const int KR = (C + 1 + 15) / 16 * 16, kr_i = KR / 16 - 1;
-  static bool attr[3][kMaxOut] = {};
-  const void* fn = kr_i == 0 ? fwd_fn<16>(O) : kr_i == 1 ? fwd_fn<32>(O) : fwd_fn<48>(O);
-  if (const char* e = set_max_smem(fn, &attr[kr_i][O - 1])) return e;
+  static bool attr[2][3][kMaxOut] = {};
+  const int pd = lim ? 1 : 0;
+  const void* fn = pd ? (kr_i == 0 ? fwd_fn<16, true>(O) : kr_i == 1 ? fwd_fn<32, true>(O) : fwd_fn<48, true>(O))
+                      : (kr_i == 0 ? fwd_fn<16, false>(O) : kr_i == 1 ? fwd_fn<32, false>(O) : fwd_fn<48, false>(O));
+  if (const char* e = set_max_smem(fn, &attr[pd][kr_i][O - 1])) return e;
   const uint32_t smem_bytes = 16384 + kStagesMF * 2 * KR * 128 + 2048 + 1024;
   const long long tiles = p.tiles_per_b * B;
   const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
-  if (kr_i == 0) launch_fwd_o<16>(O, grid, smem_bytes, stream, tmH, tmW3, p);
-  else if (kr_i == 1) launch_fwd_o<32>(O, grid, smem_bytes, stream, tmH, tmW3, p);
-  else launch_fwd_o<48>(O, grid, smem_bytes, stream, tmH, tmW3, p);
+#define DFNO_HEAD_FWD_MULTI(P_)                                                          \
+  if (kr_i == 0) launch_fwd_o<16, P_>(O, grid, smem_bytes, stream, tmH, tmW3, p, pm);      \
+  else if (kr_i == 1) launch_fwd_o<32, P_>(O, grid, smem_bytes, stream, tmH, tmW3, p, pm); \
+  else launch_fwd_o<48, P_>(O, grid, smem_bytes, stream, tmH, tmW3, p, pm);
+  if (pd) { DFNO_HEAD_FWD_MULTI(true) } else { DFNO_HEAD_FWD_MULTI(false) }
+#undef DFNO_HEAD_FWD_MULTI
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
@@ -569,7 +619,7 @@ const char* head_fwd_multi(const void* h, const void* W3aug, const float* w4b4, 
 const char* head_bwd_multi(const void* h, const void* W3aug, const void* W3T16, const float* W4, const float* dout,
                            long long n_dout, unsigned* amax_ws, void* g, float* gW3, float* gb3, float* gW4, float* gb4,
                            int B, int C, long long S, int O, long long plane, int nrl, const int* R,
-                           const long long* SR, int num_sms, cudaStream_t stream) {
+                           const long long* SR, const int* lim, int num_sms, cudaStream_t stream) {
   // C = 32 (KR = 48) would need more than the 240 consumer registers (ptxas keeps a stack frame): not instantiated
   if (C < 1 || C > 31) return "head_bwd_multi: 1 <= C <= 31";
   if (O < 1 || O > kMaxOut) return "head_bwd_multi: 1 <= O <= 4";
@@ -579,16 +629,20 @@ const char* head_bwd_multi(const void* h, const void* W3aug, const void* W3T16, 
   p.B = B; p.C = C; p.S = S; p.tiles_per_b = (S + 127) / 128; p.plane = plane;
   p.dout = dout; p.amax = reinterpret_cast<const float*>(amax_ws); p.W4 = W4;
   p.gW3 = gW3; p.gb3 = gb3; p.gW4 = gW4; p.gb4 = gb4;
-  if (set_rowmap(&p.map, nrl, R, SR)) return "head_bwd_multi: 1..4 row digits";
+  PadRowMap pm{};
+  if (lim ? set_padrowmap(&pm, nrl, R, SR, lim) : set_rowmap(&p.map, nrl, R, SR))
+    return lim ? "head_bwd_multi: 1..5 row digits, each bound within its radix" : "head_bwd_multi: 1..4 row digits";
   const int KR = (C + 1 + 15) / 16 * 16, kr_i = KR / 16 - 1;
   CUtensorMap tmH, tmW3, tmW3T, tmG;
   if (make_map_2d(&tmH, h, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (h) failed";
   if (make_map_2d(&tmW3, W3aug, 64, 128, 64, 64, 128)) return "tensor map (W3) failed";
   if (make_map_2d(&tmW3T, W3T16, 128, KR, 128, 64, KR)) return "tensor map (W3T) failed";
   if (make_map_2d(&tmG, g, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (g) failed";
-  static bool attr[2][kMaxOut] = {};
-  const void* fn = kr_i == 0 ? bwd_fn<16>(O) : bwd_fn<32>(O);
-  if (const char* e = set_max_smem(fn, &attr[kr_i][O - 1])) return e;
+  static bool attr[2][2][kMaxOut] = {};
+  const int pd = lim ? 1 : 0;
+  const void* fn = pd ? (kr_i == 0 ? bwd_fn<16, true>(O) : bwd_fn<32, true>(O))
+                      : (kr_i == 0 ? bwd_fn<16, false>(O) : bwd_fn<32, false>(O));
+  if (const char* e = set_max_smem(fn, &attr[pd][kr_i][O - 1])) return e;
   if (cudaMemsetAsync(amax_ws, 0, 4, stream) != cudaSuccess) return "head_bwd_multi: memset failed";
   absmax_kernel<<<num_sms * 4, 256, 0, stream>>>(dout, n_dout, amax_ws);
   const uint32_t tile_bytes = 2u * KR * 128;
@@ -600,8 +654,13 @@ const char* head_bwd_multi(const void* h, const void* W3aug, const void* W3T16, 
   if (smem_bytes > 227 * 1024) return "head_bwd_multi: shared memory";
   const long long tiles = p.tiles_per_b * B;
   const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
-  if (kr_i == 0) launch_bwd_o<16>(O, grid, smem_bytes, stream, tmH, tmW3, tmW3T, tmG, p);
-  else launch_bwd_o<32>(O, grid, smem_bytes, stream, tmH, tmW3, tmW3T, tmG, p);
+  if (pd) {
+    if (kr_i == 0) launch_bwd_o<16, true>(O, grid, smem_bytes, stream, tmH, tmW3, tmW3T, tmG, p, pm);
+    else launch_bwd_o<32, true>(O, grid, smem_bytes, stream, tmH, tmW3, tmW3T, tmG, p, pm);
+  } else {
+    if (kr_i == 0) launch_bwd_o<16, false>(O, grid, smem_bytes, stream, tmH, tmW3, tmW3T, tmG, p, pm);
+    else launch_bwd_o<32, false>(O, grid, smem_bytes, stream, tmH, tmW3, tmW3T, tmG, p, pm);
+  }
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }

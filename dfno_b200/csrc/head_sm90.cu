@@ -49,11 +49,11 @@ struct HeadFwdParams {
 
 // The epilogue works on the accumulator fragment (frag_row); the W4 dot is finished across the 4 lanes of a quad.
 
-// KR: channels + the ones row, padded to 16 (the K of the MMA)
-template <int KR>
-__global__ void __launch_bounds__(kThreadsHF, 1)
-head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
-                const HeadFwdParams p) {
+// KR: channels + the ones row, padded to 16 (the K of the MMA).  kPad: h is a zero-padded activation whose rows map
+// through pm; pad rows store nothing (p.map is not read).
+template <int KR, bool kPad>
+__device__ __forceinline__ void head_fwd_body(const CUtensorMap& tmH, const CUtensorMap& tmW3, const HeadFwdParams p,
+                                              const PadRowMap pm) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr uint32_t w3_bytes = KR > 64 ? 32768u : 16384u;  // one or two [128 hid][64] blocks
   uint8_t* s_w3 = smem;                                    // [128 hid][64] K-major block(s), column C = b3
@@ -157,8 +157,27 @@ head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__
       sum += __shfl_xor_sync(0xffffffffu, sum, 2);
       out[k] = sum;
     }
-    if (pos < p.S) p.out[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] = b4 + pick4(out, cq);
+    if constexpr (kPad) {
+      const long long o = pos < p.S ? pad_row_to_offset(pm, static_cast<uint32_t>(b * p.S + pos)) : -1;
+      if (o >= 0) p.out[o] = b4 + pick4(out, cq);
+    } else {
+      if (pos < p.S) p.out[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] = b4 + pick4(out, cq);
+    }
   }
+}
+
+template <int KR>
+__global__ void __launch_bounds__(kThreadsHF, 1)
+head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
+                const HeadFwdParams p) {
+  head_fwd_body<KR, false>(tmH, tmW3, p, PadRowMap{});
+}
+
+template <int KR>
+__global__ void __launch_bounds__(kThreadsHF, 1)
+head_fwd_pad_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
+                    const HeadFwdParams p, const __grid_constant__ PadRowMap pm) {
+  head_fwd_body<KR, true>(tmH, tmW3, p, pm);
 }
 
 // ================================================================================ backward
@@ -194,12 +213,11 @@ struct HeadBwdParams {
 // (frag_row): epilogue A turns each MMA1 half into P in registers, which feeds MMA2 as its register A operand and is
 // stored once with stmatrix for MMA3; dW4 stays in per-thread column registers until the flush; epilogue B stages
 // g as bf16 [C][128 positions] with stmatrix.trans and writes it with two TMA stores.
-// KR: channels + the ones row, padded to 16 (the N of MMA2 / MMA3 and the accumulator width)
-template <int KR>
-__global__ void __launch_bounds__(kThreadsHB, 1)
-head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
-                 const __grid_constant__ CUtensorMap tmW3T, const __grid_constant__ CUtensorMap tmG,
-                 const HeadBwdParams p) {
+// KR: channels + the ones row, padded to 16 (the N of MMA2 / MMA3 and the accumulator width).  kPad: rows map through
+// pm and pad rows read dout as 0, so g is exactly 0 there and they add nothing to dW3, db3, dW4, db4.
+template <int KR, bool kPad>
+__device__ __forceinline__ void head_bwd2_body(const CUtensorMap& tmH, const CUtensorMap& tmW3, const CUtensorMap& tmW3T,
+                                               const CUtensorMap& tmG, const HeadBwdParams p, const PadRowMap pm) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr uint32_t half_bytes = KR * 128;
   constexpr uint32_t tile_bytes = 2 * half_bytes;
@@ -357,7 +375,13 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
     const int b = static_cast<int>(tile / p.tiles_per_b);
     const long long p0 = (tile % p.tiles_per_b) * 128;
     const long long pos = p0 + my_row;
-    const float dl = pos < p.S ? p.dout[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] : 0.f;
+    float dl;
+    if constexpr (kPad) {
+      const long long o = pos < p.S ? pad_row_to_offset(pm, static_cast<uint32_t>(b * p.S + pos)) : -1;
+      dl = o >= 0 ? p.dout[o] : 0.f;
+    } else {
+      dl = pos < p.S ? p.dout[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] : 0.f;
+    }
     acc_gb4 += dl;
     float dk[4];                                     // dout of the thread's rows frag_row(q, lane, k)
 #pragma unroll
@@ -595,43 +619,70 @@ head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant_
   }
 }
 
+template <int KR>
+__global__ void __launch_bounds__(kThreadsHB, 1)
+head_bwd2_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
+                 const __grid_constant__ CUtensorMap tmW3T, const __grid_constant__ CUtensorMap tmG,
+                 const HeadBwdParams p) {
+  head_bwd2_body<KR, false>(tmH, tmW3, tmW3T, tmG, p, PadRowMap{});
+}
+
+template <int KR>
+__global__ void __launch_bounds__(kThreadsHB, 1)
+head_bwd2_pad_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
+                     const __grid_constant__ CUtensorMap tmW3T, const __grid_constant__ CUtensorMap tmG,
+                     const HeadBwdParams p, const __grid_constant__ PadRowMap pm) {
+  head_bwd2_body<KR, true>(tmH, tmW3, tmW3T, tmG, p, pm);
+}
+
 }  // namespace
 
 // h: bf16 [B*C, S] channel-major; W3aug: bf16 [128, 64] with column C = b3 ([128, 128] when C = 64); w4b4: fp32 [129]; out: fp32, addressed
-// through the row digits (row = b*S + position).
+// through the row digits (row = b*S + position).  lim (may be null): per-digit interior bounds of a zero-padded h
+// (up to 5 digits); rows beyond them are not stored.
 const char* head_fwd(const void* h, const void* W3aug, const float* w4b4, float* out, int B, int C, long long S,
-                     int nrl, const int* R, const long long* SR, int num_sms, cudaStream_t stream) {
+                     int nrl, const int* R, const long long* SR, const int* lim, int num_sms, cudaStream_t stream) {
   if (C < 1 || C > 64) return "head_fwd: 1 <= C <= 64";
   if (S % 8 || S > (1ll << 31) - 256 || static_cast<long long>(B) * S > (1ll << 31) - 256) return "head_fwd: bad slab size";
   HeadFwdParams p{};
   p.B = B; p.C = C; p.KR = (C + 1 + 15) / 16 * 16; p.S = S; p.tiles_per_b = (S + 127) / 128;
   p.w4b4 = w4b4; p.out = out;
-  if (set_rowmap(&p.map, nrl, R, SR)) return "head_fwd: 1..4 row digits";
+  PadRowMap pm{};
+  if (lim ? set_padrowmap(&pm, nrl, R, SR, lim) : set_rowmap(&p.map, nrl, R, SR))
+    return lim ? "head_fwd: 1..5 row digits, each bound within its radix" : "head_fwd: 1..4 row digits";
   CUtensorMap tmH, tmW3;
   if (make_map_2d(&tmH, h, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (h) failed";
   const int w3_cols = p.KR > 64 ? 128 : 64;
   if (make_map_2d(&tmW3, W3aug, w3_cols, 128, w3_cols, 64, 128)) return "tensor map (W3) failed";
-  static bool attr[5] = {false, false, false, false, false};
-  const int kr_i = p.KR / 16 - 1;
-  const void* fns[5] = {reinterpret_cast<const void*>(head_fwd_kernel<16>),
-                        reinterpret_cast<const void*>(head_fwd_kernel<32>),
-                        reinterpret_cast<const void*>(head_fwd_kernel<48>),
-                        reinterpret_cast<const void*>(head_fwd_kernel<64>),
-                        reinterpret_cast<const void*>(head_fwd_kernel<80>)};
-  const void* fn = fns[kr_i];
-  if (!attr[kr_i]) {
+  static bool attr[2][5] = {};
+  const int kr_i = p.KR / 16 - 1, pd = lim ? 1 : 0;
+  const void* fns[2][5] = {{reinterpret_cast<const void*>(head_fwd_kernel<16>),
+                            reinterpret_cast<const void*>(head_fwd_kernel<32>),
+                            reinterpret_cast<const void*>(head_fwd_kernel<48>),
+                            reinterpret_cast<const void*>(head_fwd_kernel<64>),
+                            reinterpret_cast<const void*>(head_fwd_kernel<80>)},
+                           {reinterpret_cast<const void*>(head_fwd_pad_kernel<16>),
+                            reinterpret_cast<const void*>(head_fwd_pad_kernel<32>),
+                            reinterpret_cast<const void*>(head_fwd_pad_kernel<48>),
+                            reinterpret_cast<const void*>(head_fwd_pad_kernel<64>),
+                            reinterpret_cast<const void*>(head_fwd_pad_kernel<80>)}};
+  const void* fn = fns[pd][kr_i];
+  if (!attr[pd][kr_i]) {
     if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
       return "cudaFuncSetAttribute failed";
-    attr[kr_i] = true;
+    attr[pd][kr_i] = true;
   }
   const uint32_t smem_bytes = (p.KR > 64 ? 32768 : 16384) + kStagesHF * 2 * p.KR * 128 + 2048 + 1024;
   const long long tiles = p.tiles_per_b * B;
   const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
-  if (kr_i == 0) head_fwd_kernel<16><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
-  else if (kr_i == 1) head_fwd_kernel<32><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
-  else if (kr_i == 2) head_fwd_kernel<48><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
-  else if (kr_i == 3) head_fwd_kernel<64><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
-  else head_fwd_kernel<80><<<grid, kThreadsHF, smem_bytes, stream>>>(tmH, tmW3, p);
+#define DFNO_HEAD_FWD(K_, ...)                                                                         \
+  if (kr_i == 0) K_<16><<<grid, kThreadsHF, smem_bytes, stream>>>(__VA_ARGS__);                          \
+  else if (kr_i == 1) K_<32><<<grid, kThreadsHF, smem_bytes, stream>>>(__VA_ARGS__);                     \
+  else if (kr_i == 2) K_<48><<<grid, kThreadsHF, smem_bytes, stream>>>(__VA_ARGS__);                     \
+  else if (kr_i == 3) K_<64><<<grid, kThreadsHF, smem_bytes, stream>>>(__VA_ARGS__);                     \
+  else K_<80><<<grid, kThreadsHF, smem_bytes, stream>>>(__VA_ARGS__);
+  if (pd) { DFNO_HEAD_FWD(head_fwd_pad_kernel, tmH, tmW3, p, pm) } else { DFNO_HEAD_FWD(head_fwd_kernel, tmH, tmW3, p) }
+#undef DFNO_HEAD_FWD
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
@@ -640,33 +691,40 @@ const char* head_fwd(const void* h, const void* W3aug, const float* w4b4, float*
 // (receives max |dout|); g: bf16 [B*C, S]; gradients are accumulated with atomics.
 const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const float* W4, const float* dout,
                       long long n_dout, unsigned* amax_ws, void* g, float* gW3, float* gb3, float* gW4, float* gb4,
-                      int B, int C, long long S, int nrl, const int* R, const long long* SR, int num_sms,
-                      cudaStream_t stream) {
+                      int B, int C, long long S, int nrl, const int* R, const long long* SR, const int* lim,
+                      int num_sms, cudaStream_t stream) {
   if (C < 1 || C > 64) return "head_bwd: 1 <= C <= 64";
   if (S % 8 || S > (1ll << 31) - 256 || static_cast<long long>(B) * S > (1ll << 31) - 256) return "head_bwd: bad slab size";
   HeadBwdParams p{};
   p.B = B; p.C = C; p.KR = (C + 1 + 15) / 16 * 16; p.S = S; p.tiles_per_b = (S + 127) / 128;
   p.dout = dout; p.amax = reinterpret_cast<const float*>(amax_ws); p.W4 = W4;
   p.gW3 = gW3; p.gb3 = gb3; p.gW4 = gW4; p.gb4 = gb4;
-  if (set_rowmap(&p.map, nrl, R, SR)) return "head_bwd: 1..4 row digits";
+  PadRowMap pm{};
+  if (lim ? set_padrowmap(&pm, nrl, R, SR, lim) : set_rowmap(&p.map, nrl, R, SR))
+    return lim ? "head_bwd: 1..5 row digits, each bound within its radix" : "head_bwd: 1..4 row digits";
   CUtensorMap tmH, tmW3, tmW3T, tmG;
   if (make_map_2d(&tmH, h, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (h) failed";
   const int w3_cols = p.KR > 64 ? 128 : 64;
   if (make_map_2d(&tmW3, W3aug, w3_cols, 128, w3_cols, 64, 128)) return "tensor map (W3) failed";
   if (make_map_2d(&tmW3T, W3T16, 128, p.KR, 128, 64, p.KR)) return "tensor map (W3T) failed";
   if (make_map_2d(&tmG, g, S, static_cast<uint64_t>(B) * C, S, 64, C)) return "tensor map (g) failed";
-  static bool attr[5] = {false, false, false, false, false};
-  const int kr_i = p.KR / 16 - 1;
-  const void* fns[5] = {reinterpret_cast<const void*>(head_bwd2_kernel<16>),
-                        reinterpret_cast<const void*>(head_bwd2_kernel<32>),
-                        reinterpret_cast<const void*>(head_bwd2_kernel<48>),
-                        reinterpret_cast<const void*>(head_bwd2_kernel<64>),
-                        reinterpret_cast<const void*>(head_bwd2_kernel<80>)};
-  const void* fn = fns[kr_i];
-  if (!attr[kr_i]) {
+  static bool attr[2][5] = {};
+  const int kr_i = p.KR / 16 - 1, pd = lim ? 1 : 0;
+  const void* fns[2][5] = {{reinterpret_cast<const void*>(head_bwd2_kernel<16>),
+                            reinterpret_cast<const void*>(head_bwd2_kernel<32>),
+                            reinterpret_cast<const void*>(head_bwd2_kernel<48>),
+                            reinterpret_cast<const void*>(head_bwd2_kernel<64>),
+                            reinterpret_cast<const void*>(head_bwd2_kernel<80>)},
+                           {reinterpret_cast<const void*>(head_bwd2_pad_kernel<16>),
+                            reinterpret_cast<const void*>(head_bwd2_pad_kernel<32>),
+                            reinterpret_cast<const void*>(head_bwd2_pad_kernel<48>),
+                            reinterpret_cast<const void*>(head_bwd2_pad_kernel<64>),
+                            reinterpret_cast<const void*>(head_bwd2_pad_kernel<80>)}};
+  const void* fn = fns[pd][kr_i];
+  if (!attr[pd][kr_i]) {
     if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
       return "cudaFuncSetAttribute failed";
-    attr[kr_i] = true;
+    attr[pd][kr_i] = true;
   }
   if (cudaMemsetAsync(amax_ws, 0, 4, stream) != cudaSuccess) return "head_bwd: memset failed";
   absmax_kernel<<<num_sms * 4, 256, 0, stream>>>(dout, n_dout, amax_ws);
@@ -681,11 +739,15 @@ const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const
   const uint32_t smem_bytes = fixed + p.stages * tile_bytes;
   const long long tiles = p.tiles_per_b * B;
   const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
-  if (kr_i == 0) head_bwd2_kernel<16><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
-  else if (kr_i == 1) head_bwd2_kernel<32><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
-  else if (kr_i == 2) head_bwd2_kernel<48><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
-  else if (kr_i == 3) head_bwd2_kernel<64><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
-  else head_bwd2_kernel<80><<<grid, kThreadsHB, smem_bytes, stream>>>(tmH, tmW3, tmW3T, tmG, p);
+#define DFNO_HEAD_BWD(K_, ...)                                                                         \
+  if (kr_i == 0) K_<16><<<grid, kThreadsHB, smem_bytes, stream>>>(__VA_ARGS__);                          \
+  else if (kr_i == 1) K_<32><<<grid, kThreadsHB, smem_bytes, stream>>>(__VA_ARGS__);                     \
+  else if (kr_i == 2) K_<48><<<grid, kThreadsHB, smem_bytes, stream>>>(__VA_ARGS__);                     \
+  else if (kr_i == 3) K_<64><<<grid, kThreadsHB, smem_bytes, stream>>>(__VA_ARGS__);                     \
+  else K_<80><<<grid, kThreadsHB, smem_bytes, stream>>>(__VA_ARGS__);
+  if (pd) { DFNO_HEAD_BWD(head_bwd2_pad_kernel, tmH, tmW3, tmW3T, tmG, p, pm) }
+  else { DFNO_HEAD_BWD(head_bwd2_kernel, tmH, tmW3, tmW3T, tmG, p) }
+#undef DFNO_HEAD_BWD
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }

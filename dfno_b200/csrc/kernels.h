@@ -12,12 +12,20 @@ struct LiftDims {
   int X, Y, Z;         // local spatial extents
 };
 
+// Extents of a zero-padded engine activation (each >= the LiftDims one, Z a multiple of 8): h[B*C, X, Y, T, Z] with
+// the interior [0, d.X) x [0, d.Y) x [0, d.T) x [0, d.Z) and zeros elsewhere.
+struct LiftPad {
+  int X, Y, Z, T;
+};
+
+// pad (may be null): h has the padded extents; the lift writes its pad positions as exact zeros
 const char* lift_fwd(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
-                     const float* b2, void* h, LiftDims d, int num_sms, cudaStream_t s);
-// dx (may be null): fp32 input gradient in x's layout, written (not accumulated)
+                     const float* b2, void* h, LiftDims d, const LiftPad* pad, int num_sms, cudaStream_t s);
+// dx (may be null): fp32 input gradient in x's layout, written (not accumulated).  pad (may be null): dh has the
+// padded extents and is read at interior positions only.
 const char* lift_bwd(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
                      const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2, float* dx,
-                     LiftDims d, int num_sms, cudaStream_t s);
+                     LiftDims d, const LiftPad* pad, int num_sms, cudaStream_t s);
 // strided permutation of 32-bit words: dst walked in mixed-radix order (innermost digit first, strides in words)
 const char* permute_u32(const void* src, void* dst, int nd, const int* size, const long long* sstr,
                         const long long* dstr, int num_sms, cudaStream_t s);
@@ -101,21 +109,22 @@ const char* spectral_out(const void* U, const void* h, const void* Bop, int n_pa
 // dpre = g * gelu'(pre) (in place over pre); dW += dpre . h^T
 const char* dpre_dw(const void* g, void* pre_dpre, const void* h, float* dW, int B, int C, long long L, int Z,
                     int num_sms, cudaStream_t stream);
-// projection head on the channel-major activation (head_sm90.cu)
+// projection head on the channel-major activation (head_sm90.cu).  lim (may be null): h is zero-padded; the row digits
+// (up to 5) come with per-digit interior bounds, pad rows store no output and read dout as 0.
 const char* head_fwd(const void* h, const void* W3aug, const float* w4b4, float* out, int B, int C, long long S,
-                     int nrl, const int* R, const long long* SR, int num_sms, cudaStream_t stream);
+                     int nrl, const int* R, const long long* SR, const int* lim, int num_sms, cudaStream_t stream);
 const char* head_bwd2(const void* h, const void* W3aug, const void* W3T16, const float* W4, const float* dout,
                       long long n_dout, unsigned* amax_ws, void* g, float* gW3, float* gb3, float* gW4, float* gb4,
-                      int B, int C, long long S, int nrl, const int* R, const long long* SR, int num_sms,
-                      cudaStream_t stream);
+                      int B, int C, long long S, int nrl, const int* R, const long long* SR, const int* lim,
+                      int num_sms, cudaStream_t stream);
 // projection head with O = 1..4 output channels (head_multi_sm90.cu): output channel o of a row at + o*plane.
 // w4b4 = [W4 (O x 128), b4 (O)]; the backward takes C <= 31 and reduces |dout| over all n_dout elements.
 const char* head_fwd_multi(const void* h, const void* W3aug, const float* w4b4, float* out, int B, int C, long long S,
-                           int O, long long plane, int nrl, const int* R, const long long* SR, int num_sms,
-                           cudaStream_t stream);
+                           int O, long long plane, int nrl, const int* R, const long long* SR, const int* lim,
+                           int num_sms, cudaStream_t stream);
 const char* head_bwd_multi(const void* h, const void* W3aug, const void* W3T16, const float* W4, const float* dout,
                            long long n_dout, unsigned* amax_ws, void* g, float* gW3, float* gb3, float* gW4, float* gb4,
                            int B, int C, long long S, int O, long long plane, int nrl, const int* R,
-                           const long long* SR, int num_sms, cudaStream_t stream);
+                           const long long* SR, const int* lim, int num_sms, cudaStream_t stream);
 
 }  // namespace dfno

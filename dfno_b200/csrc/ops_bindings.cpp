@@ -25,10 +25,17 @@ void* bptr(const at::Tensor& t) {
 }
 
 dfno::LiftDims lift_dims(const std::vector<int64_t>& d) {
-  TORCH_CHECK(d.size() == 8, "dims = [B, Cin, Tin, C, T, X, Y, Z]");
+  TORCH_CHECK(d.size() == 8 || d.size() == 12, "dims = [B, Cin, Tin, C, T, X, Y, Z] (+ padded [X, Y, Z, T])");
   dfno::LiftDims L;
   L.B = d[0]; L.Cin = d[1]; L.Tin = d[2]; L.C = d[3]; L.T = d[4]; L.X = d[5]; L.Y = d[6]; L.Z = d[7];
   return L;
+}
+
+// the padded extents of h when dims carries them (12 entries), else none
+const dfno::LiftPad* lift_pad(const std::vector<int64_t>& d, dfno::LiftPad* buf) {
+  if (d.size() != 12) return nullptr;
+  buf->X = d[8]; buf->Y = d[9]; buf->Z = d[10]; buf->T = d[11];
+  return buf;
 }
 
 void lift_fwd(const at::Tensor& x, const at::Tensor& W1, const at::Tensor& b1, const at::Tensor& W2,
@@ -36,8 +43,9 @@ void lift_fwd(const at::Tensor& x, const at::Tensor& W1, const at::Tensor& b1, c
   TORCH_CHECK(x.is_cuda() && x.is_contiguous(), "x must be a contiguous CUDA tensor");
   TORCH_CHECK(x.scalar_type() == at::kFloat || x.scalar_type() == at::kBFloat16, "x must be fp32 or bf16");
   c10::cuda::CUDAGuard guard(x.device());
+  dfno::LiftPad pad;
   check(dfno::lift_fwd(x.data_ptr(), x.scalar_type() == at::kBFloat16, fptr(W1), fptr(b1), fptr(W2), fptr(b2),
-                       bptr(h), lift_dims(dims), sm_count(), cur_stream()), "lift_fwd");
+                       bptr(h), lift_dims(dims), lift_pad(dims, &pad), sm_count(), cur_stream()), "lift_fwd");
 }
 
 // dx (optional): fp32 tensor of x's size, receives the input gradient
@@ -48,9 +56,11 @@ void lift_bwd(const at::Tensor& x, const at::Tensor& W1, const at::Tensor& b1, c
   TORCH_CHECK(x.scalar_type() == at::kFloat || x.scalar_type() == at::kBFloat16, "x must be fp32 or bf16");
   TORCH_CHECK(!dx || dx->numel() == x.numel(), "dx must have as many elements as x");
   c10::cuda::CUDAGuard guard(x.device());
+  dfno::LiftPad pad;
   check(dfno::lift_bwd(x.data_ptr(), x.scalar_type() == at::kBFloat16, fptr(W1), fptr(b1), fptr(W2), fptr(b2),
                        bptr(dh), fptr_mut(gW1), fptr_mut(gb1), fptr_mut(gW2), fptr_mut(gb2),
-                       dx ? const_cast<float*>(fptr(*dx)) : nullptr, lift_dims(dims), sm_count(), cur_stream()),
+                       dx ? const_cast<float*>(fptr(*dx)) : nullptr, lift_dims(dims), lift_pad(dims, &pad), sm_count(),
+                       cur_stream()),
         "lift_bwd");
 }
 
@@ -297,72 +307,85 @@ void dpre_dw(const at::Tensor& g, at::Tensor& pre_dpre, const at::Tensor& h, at:
                       static_cast<int>(Z), sm_count(), cur_stream()), "dpre_dw");
 }
 
+// row digits (+ per-digit interior bounds of a zero-padded activation, `limits`, empty for none) -> launcher arrays
+const int* row_digits(const std::vector<int64_t>& radices, const std::vector<int64_t>& strides,
+                      const std::vector<int64_t>& limits, int* R, long long* SR, int* lim) {
+  const size_t maxd = limits.empty() ? 4 : 5;
+  TORCH_CHECK(radices.size() == strides.size() && !radices.empty() && radices.size() <= maxd,
+              limits.empty() ? "1..4 row digits" : "1..5 row digits");
+  TORCH_CHECK(limits.empty() || limits.size() == radices.size(), "one limit per row digit");
+  for (size_t i = 0; i < 5; ++i) {
+    R[i] = i < radices.size() ? static_cast<int>(radices[i]) : 1;
+    SR[i] = i < strides.size() ? strides[i] : 0;
+    lim[i] = i < limits.size() ? static_cast<int>(limits[i]) : 1;
+  }
+  return limits.empty() ? nullptr : lim;
+}
+
 void head_fwd(const at::Tensor& h, const at::Tensor& W3aug, const at::Tensor& w4b4, at::Tensor& out, int64_t B,
-              int64_t C, int64_t S, const std::vector<int64_t>& radices, const std::vector<int64_t>& strides) {
-  TORCH_CHECK(radices.size() == strides.size() && !radices.empty() && radices.size() <= 4, "1..4 row digits");
+              int64_t C, int64_t S, const std::vector<int64_t>& radices, const std::vector<int64_t>& strides,
+              const std::vector<int64_t>& limits) {
   TORCH_CHECK(W3aug.dim() == 2 && W3aug.size(0) == 128 && W3aug.size(1) == (C + 1 > 64 ? 128 : 64) &&
               W3aug.is_contiguous(), "W3aug [128, 64] ([128, 128] when C + 1 > 64)");
   TORCH_CHECK(w4b4.numel() >= 129, "w4b4 = [W4 (128), b4]");
   c10::cuda::CUDAGuard guard(h.device());
-  int R[4]; long long SR[4];
-  for (size_t i = 0; i < 4; ++i) { R[i] = i < radices.size() ? static_cast<int>(radices[i]) : 1; SR[i] = i < strides.size() ? strides[i] : 0; }
+  int R[5], lim[5]; long long SR[5];
+  const int* lp = row_digits(radices, strides, limits, R, SR, lim);
   check(dfno::head_fwd(bptr(h), bptr(W3aug), fptr(w4b4), fptr_mut(out), static_cast<int>(B), static_cast<int>(C), S,
-                       static_cast<int>(radices.size()), R, SR, sm_count(), cur_stream()), "head_fwd");
+                       static_cast<int>(radices.size()), R, SR, lp, sm_count(), cur_stream()), "head_fwd");
 }
 
 void head_bwd2(const at::Tensor& h, const at::Tensor& W3aug, const at::Tensor& W3T16, const at::Tensor& W4,
                const at::Tensor& dout, at::Tensor& amax_ws, at::Tensor& g, at::Tensor& gW3, at::Tensor& gb3,
                at::Tensor& gW4, at::Tensor& gb4, int64_t B, int64_t C, int64_t S, const std::vector<int64_t>& radices,
-               const std::vector<int64_t>& strides) {
-  TORCH_CHECK(radices.size() == strides.size() && !radices.empty() && radices.size() <= 4, "1..4 row digits");
+               const std::vector<int64_t>& strides, const std::vector<int64_t>& limits) {
   TORCH_CHECK(W3aug.dim() == 2 && W3aug.size(0) == 128 && W3aug.size(1) == (C + 1 > 64 ? 128 : 64) &&
               W3aug.is_contiguous(), "W3aug [128, 64] ([128, 128] when C + 1 > 64)");
   TORCH_CHECK(W3T16.is_cuda() && W3T16.scalar_type() == at::kHalf && W3T16.dim() == 2 && W3T16.size(1) == 128 &&
               W3T16.size(0) == (C + 1 + 15) / 16 * 16 && W3T16.is_contiguous(), "W3T16: fp16 [ceil16(C+1), 128]");
   TORCH_CHECK(amax_ws.is_cuda() && amax_ws.numel() >= 1 && amax_ws.element_size() == 4, "amax_ws: one 32-bit word");
   c10::cuda::CUDAGuard guard(h.device());
-  int R[4]; long long SR[4];
-  for (size_t i = 0; i < 4; ++i) { R[i] = i < radices.size() ? static_cast<int>(radices[i]) : 1; SR[i] = i < strides.size() ? strides[i] : 0; }
+  int R[5], lim[5]; long long SR[5];
+  const int* lp = row_digits(radices, strides, limits, R, SR, lim);
   check(dfno::head_bwd2(bptr(h), bptr(W3aug), W3T16.data_ptr(), fptr(W4), fptr(dout), dout.numel(),
                         reinterpret_cast<unsigned*>(amax_ws.data_ptr()), bptr(g), fptr_mut(gW3), fptr_mut(gb3),
                         fptr_mut(gW4), fptr_mut(gb4), static_cast<int>(B), static_cast<int>(C), S,
-                        static_cast<int>(radices.size()), R, SR, sm_count(), cur_stream()), "head_bwd2");
+                        static_cast<int>(radices.size()), R, SR, lp, sm_count(), cur_stream()), "head_bwd2");
 }
 
 // out: fp32 [B, O, ...] addressed through the row digits, output channel o at + o * plane
 void head_fwd_multi(const at::Tensor& h, const at::Tensor& W3aug, const at::Tensor& w4b4, at::Tensor& out, int64_t B,
                     int64_t C, int64_t S, int64_t O, int64_t plane, const std::vector<int64_t>& radices,
-                    const std::vector<int64_t>& strides) {
-  TORCH_CHECK(radices.size() == strides.size() && !radices.empty() && radices.size() <= 4, "1..4 row digits");
+                    const std::vector<int64_t>& strides, const std::vector<int64_t>& limits) {
   TORCH_CHECK(W3aug.dim() == 2 && W3aug.size(0) == 128 && W3aug.size(1) == 64 && W3aug.is_contiguous(), "W3aug [128,64]");
   TORCH_CHECK(w4b4.numel() >= O * 129, "w4b4 = [W4 (O x 128), b4 (O)]");
-  TORCH_CHECK(out.numel() >= B * O * S, "out smaller than B * O * S");
+  TORCH_CHECK(out.numel() >= B * O * plane, "out smaller than B * O * plane");
   c10::cuda::CUDAGuard guard(h.device());
-  int R[4]; long long SR[4];
-  for (size_t i = 0; i < 4; ++i) { R[i] = i < radices.size() ? static_cast<int>(radices[i]) : 1; SR[i] = i < strides.size() ? strides[i] : 0; }
+  int R[5], lim[5]; long long SR[5];
+  const int* lp = row_digits(radices, strides, limits, R, SR, lim);
   check(dfno::head_fwd_multi(bptr(h), bptr(W3aug), fptr(w4b4), fptr_mut(out), static_cast<int>(B), static_cast<int>(C),
-                             S, static_cast<int>(O), plane, static_cast<int>(radices.size()), R, SR, sm_count(),
+                             S, static_cast<int>(O), plane, static_cast<int>(radices.size()), R, SR, lp, sm_count(),
                              cur_stream()), "head_fwd_multi");
 }
 
 void head_bwd_multi(const at::Tensor& h, const at::Tensor& W3aug, const at::Tensor& W3T16, const at::Tensor& W4,
                     const at::Tensor& dout, at::Tensor& amax_ws, at::Tensor& g, at::Tensor& gW3, at::Tensor& gb3,
                     at::Tensor& gW4, at::Tensor& gb4, int64_t B, int64_t C, int64_t S, int64_t O, int64_t plane,
-                    const std::vector<int64_t>& radices, const std::vector<int64_t>& strides) {
-  TORCH_CHECK(radices.size() == strides.size() && !radices.empty() && radices.size() <= 4, "1..4 row digits");
+                    const std::vector<int64_t>& radices, const std::vector<int64_t>& strides,
+                    const std::vector<int64_t>& limits) {
   TORCH_CHECK(W3aug.dim() == 2 && W3aug.size(0) == 128 && W3aug.size(1) == 64 && W3aug.is_contiguous(), "W3aug [128,64]");
   TORCH_CHECK(W3T16.is_cuda() && W3T16.scalar_type() == at::kHalf && W3T16.dim() == 2 && W3T16.size(1) == 128 &&
               W3T16.size(0) == (C + 1 + 15) / 16 * 16 && W3T16.is_contiguous(), "W3T16: fp16 [ceil16(C+1), 128]");
   TORCH_CHECK(W4.numel() == O * 128 && gW4.numel() == O * 128 && gb4.numel() == O, "W4 / dW4 [O, 128], db4 [O]");
-  TORCH_CHECK(dout.numel() >= B * O * S, "dout smaller than B * O * S");
+  TORCH_CHECK(dout.numel() >= B * O * plane, "dout smaller than B * O * plane");
   TORCH_CHECK(amax_ws.is_cuda() && amax_ws.numel() >= 1 && amax_ws.element_size() == 4, "amax_ws: one 32-bit word");
   c10::cuda::CUDAGuard guard(h.device());
-  int R[4]; long long SR[4];
-  for (size_t i = 0; i < 4; ++i) { R[i] = i < radices.size() ? static_cast<int>(radices[i]) : 1; SR[i] = i < strides.size() ? strides[i] : 0; }
+  int R[5], lim[5]; long long SR[5];
+  const int* lp = row_digits(radices, strides, limits, R, SR, lim);
   check(dfno::head_bwd_multi(bptr(h), bptr(W3aug), W3T16.data_ptr(), fptr(W4), fptr(dout), dout.numel(),
                              reinterpret_cast<unsigned*>(amax_ws.data_ptr()), bptr(g), fptr_mut(gW3), fptr_mut(gb3),
                              fptr_mut(gW4), fptr_mut(gb4), static_cast<int>(B), static_cast<int>(C), S,
-                             static_cast<int>(O), plane, static_cast<int>(radices.size()), R, SR, sm_count(),
+                             static_cast<int>(O), plane, static_cast<int>(radices.size()), R, SR, lp, sm_count(),
                              cur_stream()), "head_bwd_multi");
 }
 
@@ -377,10 +400,19 @@ void register_ops(pybind11::module& m) {
   m.def("spectral_in_config", &spectral_in_config);
   m.def("spectral_out", &spectral_out);
   m.def("dpre_dw", &dpre_dw);
-  m.def("head_fwd", &head_fwd);
-  m.def("head_bwd2", &head_bwd2);
-  m.def("head_fwd_multi", &head_fwd_multi);
-  m.def("head_bwd_multi", &head_bwd_multi);
+  // limits (optional): per-digit interior bounds of a zero-padded h
+  m.def("head_fwd", &head_fwd, py::arg("h"), py::arg("W3aug"), py::arg("w4b4"), py::arg("out"), py::arg("B"), py::arg("C"),
+        py::arg("S"), py::arg("radices"), py::arg("strides"), py::arg("limits") = std::vector<int64_t>{});
+  m.def("head_bwd2", &head_bwd2, py::arg("h"), py::arg("W3aug"), py::arg("W3T16"), py::arg("W4"), py::arg("dout"),
+        py::arg("amax_ws"), py::arg("g"), py::arg("gW3"), py::arg("gb3"), py::arg("gW4"), py::arg("gb4"), py::arg("B"),
+        py::arg("C"), py::arg("S"), py::arg("radices"), py::arg("strides"), py::arg("limits") = std::vector<int64_t>{});
+  m.def("head_fwd_multi", &head_fwd_multi, py::arg("h"), py::arg("W3aug"), py::arg("w4b4"), py::arg("out"), py::arg("B"),
+        py::arg("C"), py::arg("S"), py::arg("O"), py::arg("plane"), py::arg("radices"), py::arg("strides"),
+        py::arg("limits") = std::vector<int64_t>{});
+  m.def("head_bwd_multi", &head_bwd_multi, py::arg("h"), py::arg("W3aug"), py::arg("W3T16"), py::arg("W4"),
+        py::arg("dout"), py::arg("amax_ws"), py::arg("g"), py::arg("gW3"), py::arg("gb3"), py::arg("gW4"), py::arg("gb4"),
+        py::arg("B"), py::arg("C"), py::arg("S"), py::arg("O"), py::arg("plane"), py::arg("radices"), py::arg("strides"),
+        py::arg("limits") = std::vector<int64_t>{});
   m.def("lift_fwd", &lift_fwd);
   m.def("lift_bwd", &lift_bwd, py::arg("x"), py::arg("W1"), py::arg("b1"), py::arg("W2"), py::arg("b2"), py::arg("dh"),
         py::arg("gW1"), py::arg("gb1"), py::arg("gW2"), py::arg("gb2"), py::arg("dims"), py::arg("dx") = c10::nullopt);

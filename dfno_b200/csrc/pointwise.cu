@@ -78,11 +78,14 @@ __device__ __forceinline__ void lift_inner(const TIn* __restrict__ xci, const fl
   }
 }
 
-template <typename TIn, int CIN, bool kRegs>
-__global__ void __launch_bounds__(256)
-lift_fwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
-                const float* __restrict__ W2, const float* __restrict__ b2, __nv_bfloat16* __restrict__ h,
-                LiftDims d) {
+// kPad: h has the padded extents e (>= d's); items of the padded grid beyond d's x, y or z, and the t steps beyond
+// d.T of interior items, are written as exact zeros in the same pass (Z and e.Z multiples of 8: an item is either
+// interior or pad).  Without kPad, e is not read.
+template <typename TIn, int CIN, bool kRegs, bool kPad>
+__device__ __forceinline__ void
+lift_fwd_body(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+              const float* __restrict__ W2, const float* __restrict__ b2, __nv_bfloat16* __restrict__ h,
+              LiftDims d, LiftPad e) {
   __shared__ float sw[kLiftMaxW];
   float* sW1 = sw;                                          // [T][Tin]
   float* sb1 = sW1 + d.T * d.Tin;                           // [T]
@@ -94,14 +97,28 @@ lift_fwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
   for (int i = threadIdx.x; i < d.C; i += blockDim.x) sb2[i] = __float2half2_rn(b2[i]);
   __syncthreads();
 
-  const int zv = d.Z >> 3;
+  const int hZ = kPad ? e.Z : d.Z, hT = kPad ? e.T : d.T;   // h's z and t extents
+  const int zv = hZ >> 3;
   const long long plane = static_cast<long long>(d.X) * d.Y;
-  const long long nitems = static_cast<long long>(d.B) * plane * zv;
+  const long long hplane = kPad ? static_cast<long long>(e.X) * e.Y : plane;
+  const long long nitems = static_cast<long long>(d.B) * hplane * zv;
   for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < nitems;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int z0 = static_cast<int>(idx % zv) * 8;
-    const long long xy = (idx / zv) % plane;
-    const int b = static_cast<int>(idx / (zv * plane));
+    const long long hxy = (idx / zv) % hplane;
+    const int b = static_cast<int>(idx / (zv * hplane));
+    long long xy = hxy;
+    if constexpr (kPad) {
+      const int px = static_cast<int>(hxy / e.Y), py = static_cast<int>(hxy % e.Y);
+      if (px >= d.X || py >= d.Y || z0 >= d.Z) {
+        __nv_bfloat16* hb = h + ((static_cast<long long>(b) * d.C * hplane + hxy) * hT) * hZ + z0;
+        for (int c = 0; c < d.C; ++c)
+          for (int t = 0; t < hT; ++t)
+            *reinterpret_cast<uint4*>(hb + (c * hplane * hT + t) * hZ) = make_uint4(0, 0, 0, 0);
+        continue;
+      }
+      xy = static_cast<long long>(px) * d.Y + py;
+    }
     const TIn* xb = x + (((static_cast<long long>(b) * CIN) * plane + xy) * d.Z + z0) * d.Tin;
     const long long xci_stride = plane * d.Z * d.Tin;
     float xr[kRegs ? CIN : 1][8];
@@ -109,8 +126,13 @@ lift_fwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
 #pragma unroll
       for (int ci = 0; ci < CIN; ++ci) lift_load8<TIn>(xb + ci * xci_stride, 1, 0, xr[ci]);
     }
-    __nv_bfloat16* hb = h + ((static_cast<long long>(b) * d.C * plane + xy) * d.T) * d.Z + z0;
-    const long long hc_stride = plane * d.T * d.Z;
+    __nv_bfloat16* hb = h + ((static_cast<long long>(b) * d.C * hplane + hxy) * hT) * hZ + z0;
+    const long long hc_stride = hplane * hT * hZ;
+    if constexpr (kPad) {
+      for (int c = 0; c < d.C; ++c)
+        for (int t = d.T; t < hT; ++t)
+          *reinterpret_cast<uint4*>(hb + c * hc_stride + static_cast<long long>(t) * hZ) = make_uint4(0, 0, 0, 0);
+    }
     for (int t = 0; t < d.T; ++t) {
       __half2 a1[CIN][4];
 #pragma unroll
@@ -129,10 +151,26 @@ lift_fwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
           for (int ci = 0; ci < CIN; ++ci) acc = __hfma2(sW2[c * CIN + ci], a1[ci][k], acc);
           o[k] = h2_to_bf16x2(gelu_h2(acc));
         }
-        *reinterpret_cast<uint4*>(hb + c * hc_stride + static_cast<long long>(t) * d.Z) = make_uint4(o[0], o[1], o[2], o[3]);
+        *reinterpret_cast<uint4*>(hb + c * hc_stride + static_cast<long long>(t) * hZ) = make_uint4(o[0], o[1], o[2], o[3]);
       }
     }
   }
+}
+
+template <typename TIn, int CIN, bool kRegs>
+__global__ void __launch_bounds__(256)
+lift_fwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                const float* __restrict__ W2, const float* __restrict__ b2, __nv_bfloat16* __restrict__ h,
+                LiftDims d) {
+  lift_fwd_body<TIn, CIN, kRegs, false>(x, W1, b1, W2, b2, h, d, LiftPad{});
+}
+
+template <typename TIn, int CIN, bool kRegs>
+__global__ void __launch_bounds__(256)
+lift_fwd_pad_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                    const float* __restrict__ W2, const float* __restrict__ b2, __nv_bfloat16* __restrict__ h,
+                    LiftDims d, LiftPad e) {
+  lift_fwd_body<TIn, CIN, kRegs, true>(x, W1, b1, W2, b2, h, d, e);
 }
 
 // dW1[T][Tin], db1[T], dW2[C][Cin], db2[C] accumulated with atomics into fp32 buffers.  Four adjacent lanes share
@@ -151,12 +189,14 @@ lift_fwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
 //
 // Widths above 32 (48, 64) split the channels over eight lanes instead (kSplit): each lane keeps C/8 channel sums, the
 // per-thread register cost of width 32.  The input gradient is then written by the first four lanes of the eight.
-template <typename TIn, int C, int CIN, bool kRegs, bool kDx>
-__global__ void __launch_bounds__(128, (CIN == 1 ? 4 : 2))      // several input channels: more live values, no spills
-lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
-                const float* __restrict__ W2, const float* __restrict__ b2,
-                const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
-                float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx) {
+//
+// kPad: dh has the padded extents e; only its interior positions are read (the pad region of h is a constant).
+template <typename TIn, int C, int CIN, bool kRegs, bool kDx, bool kPad>
+__device__ __forceinline__ void
+lift_bwd_body(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+              const float* __restrict__ W2, const float* __restrict__ b2,
+              const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
+              float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx, LiftPad e) {
   constexpr int kSplitLog = C > 32 ? 3 : 2;
   constexpr int kSplit = 1 << kSplitLog;                     // lanes per item
   static_assert(C % kSplit == 0, "the channels are split evenly over the lanes of an item");
@@ -206,8 +246,11 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
 #pragma unroll
       for (int ci = 0; ci < CIN; ++ci) lift_load8<TIn>(xb + ci * xci_stride, 1, 0, xr[ci]);
     }
-    const long long hc_stride = plane * d.T * d.Z;
-    const __nv_bfloat16* gb = dh + ((static_cast<long long>(b) * C * plane + xy) * d.T) * d.Z + z0 + c0 * hc_stride;
+    const int hZ = kPad ? e.Z : d.Z, hT = kPad ? e.T : d.T;
+    const long long hplane = kPad ? static_cast<long long>(e.X) * e.Y : plane;
+    const long long hxy = kPad ? (xy / d.Y) * e.Y + xy % d.Y : xy;
+    const long long hc_stride = hplane * hT * hZ;
+    const __nv_bfloat16* gb = dh + ((static_cast<long long>(b) * C * hplane + hxy) * hT) * hZ + z0 + c0 * hc_stride;
     float* dxl = kDx ? dx + (xb - x) + 2 * cg * d.Tin : nullptr;     // this lane's run [2 z][Tin] of ci = 0
     float dxr[kDx && kRegs ? CIN : 1][2];
     if (kDx && kRegs) {
@@ -234,7 +277,7 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
       uint4 gv[CG];                                         // this lane's channel loads, all in flight together
 #pragma unroll
       for (int u = 0; u < CG; ++u)
-        gv[u] = ok ? *reinterpret_cast<const uint4*>(gb + u * hc_stride + static_cast<long long>(t) * d.Z)
+        gv[u] = ok ? *reinterpret_cast<const uint4*>(gb + u * hc_stride + static_cast<long long>(t) * hZ)
                    : make_uint4(0, 0, 0, 0);
 #pragma unroll
       for (int u = 0; u < CG; ++u) {
@@ -358,6 +401,24 @@ lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const f
   for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(&gb2[i], gsW2[C * CIN + i]);
 }
 
+template <typename TIn, int C, int CIN, bool kRegs, bool kDx>
+__global__ void __launch_bounds__(128, (CIN == 1 ? 4 : 2))      // several input channels: more live values, no spills
+lift_bwd_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                const float* __restrict__ W2, const float* __restrict__ b2,
+                const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
+                float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx) {
+  lift_bwd_body<TIn, C, CIN, kRegs, kDx, false>(x, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, d, dx, LiftPad{});
+}
+
+template <typename TIn, int C, int CIN, bool kRegs, bool kDx>
+__global__ void __launch_bounds__(128, (CIN == 1 ? 4 : 2))
+lift_bwd_pad_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                    const float* __restrict__ W2, const float* __restrict__ b2,
+                    const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
+                    float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx, LiftPad e) {
+  lift_bwd_body<TIn, C, CIN, kRegs, kDx, true>(x, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, d, dx, e);
+}
+
 // ------------------------------------------------------------------------------------------
 // lift, 5 <= Cin <= 16
 // ------------------------------------------------------------------------------------------
@@ -424,11 +485,12 @@ __device__ __forceinline__ void lift_many_inner(const TIn* __restrict__ xz, cons
   }
 }
 
-template <typename TIn, int CINP, bool kRegs>
-__global__ void __launch_bounds__(32 * kLiftManyWarps)
-lift_fwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
-                     const float* __restrict__ W2, const float* __restrict__ b2, __nv_bfloat16* __restrict__ h,
-                     LiftDims d) {
+// kPad: as lift_fwd_kernel (pad items and t steps written as zeros by the lanes of the channel phase)
+template <typename TIn, int CINP, bool kRegs, bool kPad>
+__device__ __forceinline__ void
+lift_fwd_many_body(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                   const float* __restrict__ W2, const float* __restrict__ b2, __nv_bfloat16* __restrict__ h,
+                   LiftDims d, LiftPad e) {
   using L = LiftManyLanes<CINP>;
   constexpr int ZL = L::ZL, kWarps = kLiftManyWarps;
   extern __shared__ uint4 fxs[];                                       // per warp: Cin runs of x (Tin > 1)
@@ -450,15 +512,28 @@ lift_fwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, co
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ci = lane / L::kParts, zl = (lane % L::kParts) * ZL;        // input-side role
   const bool live = ci < d.Cin;
-  const int zv = d.Z >> 3;
+  const int hZ = kPad ? e.Z : d.Z, hT = kPad ? e.T : d.T;   // h's z and t extents
+  const int zv = hZ >> 3;
   const long long plane = static_cast<long long>(d.X) * d.Y;
-  const long long nitems = static_cast<long long>(d.B) * plane * zv;
-  const long long hc_stride = plane * d.T * d.Z;
+  const long long hplane = kPad ? static_cast<long long>(e.X) * e.Y : plane;
+  const long long nitems = static_cast<long long>(d.B) * hplane * zv;
+  const long long hc_stride = hplane * hT * hZ;
   for (long long idx = blockIdx.x * static_cast<long long>(kWarps) + warp; idx < nitems;
        idx += static_cast<long long>(gridDim.x) * kWarps) {              // warp-uniform
     const int z0 = static_cast<int>(idx % zv) * 8;
-    const long long xy = (idx / zv) % plane;
-    const int b = static_cast<int>(idx / (zv * plane));
+    const long long hxy = (idx / zv) % hplane;
+    const int b = static_cast<int>(idx / (zv * hplane));
+    __nv_bfloat16* hb = h + ((static_cast<long long>(b) * d.C * hplane + hxy) * hT) * hZ + z0;
+    long long xy = hxy;
+    if constexpr (kPad) {
+      const int px = static_cast<int>(hxy / e.Y), py = static_cast<int>(hxy % e.Y);
+      const bool pad = px >= d.X || py >= d.Y || z0 >= d.Z;
+      for (int c = lane; c < d.C; c += 32)
+        for (int t = pad ? 0 : d.T; t < hT; ++t)
+          *reinterpret_cast<uint4*>(hb + c * hc_stride + static_cast<long long>(t) * hZ) = make_uint4(0, 0, 0, 0);
+      if (pad) continue;
+      xy = static_cast<long long>(px) * d.Y + py;
+    }
     const TIn* xb = x + ((static_cast<long long>(b) * d.Cin * plane + xy) * d.Z + z0) * d.Tin;
     const long long xci_stride = plane * d.Z * d.Tin;
     const TIn* xz;
@@ -473,7 +548,6 @@ lift_fwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, co
       __syncwarp();
       xz = xs + (live ? ci : 0) * xss + zl * d.Tin;
     }
-    __nv_bfloat16* hb = h + ((static_cast<long long>(b) * d.C * plane + xy) * d.T) * d.Z + z0;
     for (int t = 0; t < d.T; ++t) {
       float v[ZL];
       if (live) lift_many_inner<TIn, ZL, kRegs>(xz, xr, d.Tin, sW1 + t * d.Tin, sb1[t], v);
@@ -497,11 +571,27 @@ lift_fwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, co
         uint32_t o[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) o[k] = h2_to_bf16x2(gelu_h2(acc[k]));
-        *reinterpret_cast<uint4*>(hb + c * hc_stride + static_cast<long long>(t) * d.Z) = make_uint4(o[0], o[1], o[2], o[3]);
+        *reinterpret_cast<uint4*>(hb + c * hc_stride + static_cast<long long>(t) * hZ) = make_uint4(o[0], o[1], o[2], o[3]);
       }
       __syncwarp();
     }
   }
+}
+
+template <typename TIn, int CINP, bool kRegs>
+__global__ void __launch_bounds__(32 * kLiftManyWarps)
+lift_fwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                     const float* __restrict__ W2, const float* __restrict__ b2, __nv_bfloat16* __restrict__ h,
+                     LiftDims d) {
+  lift_fwd_many_body<TIn, CINP, kRegs, false>(x, W1, b1, W2, b2, h, d, LiftPad{});
+}
+
+template <typename TIn, int CINP, bool kRegs>
+__global__ void __launch_bounds__(32 * kLiftManyWarps)
+lift_fwd_many_pad_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                         const float* __restrict__ W2, const float* __restrict__ b2, __nv_bfloat16* __restrict__ h,
+                         LiftDims d, LiftPad e) {
+  lift_fwd_many_body<TIn, CINP, kRegs, true>(x, W1, b1, W2, b2, h, d, e);
 }
 
 // Backward of lift_fwd_many_kernel: the same outputs as lift_bwd_kernel.  Per t, after the time lift:
@@ -512,13 +602,13 @@ lift_fwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, co
 //                db1[t], dW1[t, :] (warp sums) and, with kDx, its own dx values: Tin == 1 keeps them in registers
 //                over t, otherwise the first t stores and later t add (read-modify-write of the lane's own values).
 // Everything the loss gradient multiplies is fp32; the GELU' evaluations are packed fp16.  W1 / b1 and their
-// gradient sums take dynamic shared memory (2 * (T * Tin + T) floats).
-template <typename TIn, int CINP, bool kRegs, bool kDx>
-__global__ void __launch_bounds__(32 * kLiftManyWarps, (CINP == 8 ? 4 : 3))        // 16 channels: more live values, no spills
-lift_bwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
-                     const float* __restrict__ W2, const float* __restrict__ b2,
-                     const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
-                     float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx) {
+// gradient sums take dynamic shared memory (2 * (T * Tin + T) floats).  kPad: as lift_bwd_kernel.
+template <typename TIn, int CINP, bool kRegs, bool kDx, bool kPad>
+__device__ __forceinline__ void
+lift_bwd_many_body(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                   const float* __restrict__ W2, const float* __restrict__ b2,
+                   const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
+                   float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx, LiftPad e) {
   using L = LiftManyLanes<CINP>;
   constexpr int ZL = L::ZL, kWarps = kLiftManyWarps, kU = kLiftManyMaxC / 32;
   extern __shared__ float dsm[];                                       // W1, b1, their sums; then the x slices
@@ -554,12 +644,15 @@ lift_bwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, co
   const int zv = d.Z >> 3;
   const long long plane = static_cast<long long>(d.X) * d.Y;
   const long long nitems = static_cast<long long>(d.B) * plane * zv;
-  const long long hc_stride = plane * d.T * d.Z;
+  const int hZ = kPad ? e.Z : d.Z, hT = kPad ? e.T : d.T;
+  const long long hplane = kPad ? static_cast<long long>(e.X) * e.Y : plane;
+  const long long hc_stride = hplane * hT * hZ;
   for (long long idx = blockIdx.x * static_cast<long long>(kWarps) + warp; idx < nitems;
        idx += static_cast<long long>(gridDim.x) * kWarps) {              // warp-uniform
     const int z0 = static_cast<int>(idx % zv) * 8;
     const long long xy = (idx / zv) % plane;
     const int b = static_cast<int>(idx / (zv * plane));
+    const long long hxy = kPad ? (xy / d.Y) * e.Y + xy % d.Y : xy;
     const long long xoff = ((((static_cast<long long>(b) * d.Cin) + (live ? ci : 0)) * plane + xy) * d.Z + z0 + zl) * d.Tin;
     const TIn* xz;
     float xr[ZL];
@@ -575,7 +668,7 @@ lift_bwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, co
       __syncwarp();
       xz = xs + (live ? ci : 0) * xss + zl * d.Tin;
     }
-    const __nv_bfloat16* gb = dh + ((static_cast<long long>(b) * d.C * plane + xy) * d.T) * d.Z + z0;
+    const __nv_bfloat16* gb = dh + ((static_cast<long long>(b) * d.C * hplane + hxy) * hT) * hZ + z0;
     float dxr[ZL];
 #pragma unroll
     for (int z = 0; z < ZL; ++z) dxr[z] = 0.f;
@@ -599,7 +692,7 @@ lift_bwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, co
       for (int u = 0; u < kU; ++u) {
         const int c = lane + 32 * u;
         if (c < d.C) {
-          const uint4 gw = *reinterpret_cast<const uint4*>(gb + c * hc_stride + static_cast<long long>(t) * d.Z);
+          const uint4 gw = *reinterpret_cast<const uint4*>(gb + c * hc_stride + static_cast<long long>(t) * hZ);
           __half2 acc[4];
 #pragma unroll
           for (int k = 0; k < 4; ++k) acc[k] = sb2[c];
@@ -711,6 +804,25 @@ lift_bwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, co
   for (int i = threadIdx.x; i < d.T; i += blockDim.x) atomicAdd(&gb1[i], gsb1[i]);
   for (int i = threadIdx.x; i < d.C * d.Cin; i += blockDim.x) atomicAdd(&gW2[i], gsW2[(i / d.Cin) * CINP + i % d.Cin]);
   for (int i = threadIdx.x; i < d.C; i += blockDim.x) atomicAdd(&gb2[i], gsW2[d.C * CINP + i]);
+}
+
+template <typename TIn, int CINP, bool kRegs, bool kDx>
+__global__ void __launch_bounds__(32 * kLiftManyWarps, (CINP == 8 ? 4 : 3))        // 16 channels: more live values, no spills
+lift_bwd_many_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                     const float* __restrict__ W2, const float* __restrict__ b2,
+                     const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
+                     float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx) {
+  lift_bwd_many_body<TIn, CINP, kRegs, kDx, false>(x, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, d, dx, LiftPad{});
+}
+
+template <typename TIn, int CINP, bool kRegs, bool kDx>
+__global__ void __launch_bounds__(32 * kLiftManyWarps, (CINP == 8 ? 4 : 3))
+lift_bwd_many_pad_kernel(const TIn* __restrict__ x, const float* __restrict__ W1, const float* __restrict__ b1,
+                         const float* __restrict__ W2, const float* __restrict__ b2,
+                         const __nv_bfloat16* __restrict__ dh, float* __restrict__ gW1, float* __restrict__ gb1,
+                         float* __restrict__ gW2, float* __restrict__ gb2, LiftDims d, float* __restrict__ dx,
+                         LiftPad e) {
+  lift_bwd_many_body<TIn, CINP, kRegs, kDx, true>(x, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, d, dx, e);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -967,8 +1079,10 @@ const char* gelu_probe(const float* x, float* y, float* dy, long long n, cudaStr
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
-static const char* lift_check(const LiftDims& d) {
+static const char* lift_check(const LiftDims& d, const LiftPad* pad) {
   if (d.Z % 8) return "lift: Z must be a multiple of 8";
+  if (pad && (pad->X < d.X || pad->Y < d.Y || pad->Z < d.Z || pad->T < d.T || pad->Z % 8))
+    return "lift: padded extents must be >= the interior ones, padded Z a multiple of 8";
   if (d.Cin < 1 || d.Cin > 16) return "lift: supported input channel counts are 1..16";
   if (d.Tin < 1 || d.Tin > kLiftMaxTin) return "lift: 1 <= Tin <= 64";
   if (d.C > 64) return "lift: C <= 64";
@@ -993,61 +1107,83 @@ static const char* lift_many_allow_smem(K kern, bool& done, size_t bytes) {
   return nullptr;
 }
 
-template <typename TIn, int CINP, bool kRegs>
+template <typename TIn, int CINP, bool kRegs, bool kPad>
 static const char* lift_fwd_many_launch(const void* x, const float* W1, const float* b1, const float* W2,
-                                        const float* b2, void* h, LiftDims d, int grid, cudaStream_t s) {
-  auto kern = lift_fwd_many_kernel<TIn, CINP, kRegs>;
+                                        const float* b2, void* h, LiftDims d, LiftPad ep, int grid, cudaStream_t s) {
   static bool attr = false;
-  if (const char* e = lift_many_allow_smem(kern, attr, lift_many_xs_bytes<TIn>(16, kLiftMaxTin))) return e;
-  kern<<<grid, 32 * kLiftManyWarps, lift_many_xs_bytes<TIn>(d.Cin, d.Tin), s>>>(
-      static_cast<const TIn*>(x), W1, b1, W2, b2, static_cast<__nv_bfloat16*>(h), d);
+  const size_t smem = lift_many_xs_bytes<TIn>(d.Cin, d.Tin);
+  if constexpr (kPad) {
+    auto kern = lift_fwd_many_pad_kernel<TIn, CINP, kRegs>;
+    if (const char* e = lift_many_allow_smem(kern, attr, lift_many_xs_bytes<TIn>(16, kLiftMaxTin))) return e;
+    kern<<<grid, 32 * kLiftManyWarps, smem, s>>>(static_cast<const TIn*>(x), W1, b1, W2, b2,
+                                                 static_cast<__nv_bfloat16*>(h), d, ep);
+  } else {
+    auto kern = lift_fwd_many_kernel<TIn, CINP, kRegs>;
+    if (const char* e = lift_many_allow_smem(kern, attr, lift_many_xs_bytes<TIn>(16, kLiftMaxTin))) return e;
+    kern<<<grid, 32 * kLiftManyWarps, smem, s>>>(static_cast<const TIn*>(x), W1, b1, W2, b2,
+                                                 static_cast<__nv_bfloat16*>(h), d);
+  }
   return nullptr;
 }
 
 static const char* lift_fwd_many(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
-                                 const float* b2, void* h, LiftDims d, int num_sms, cudaStream_t s) {
-  const long long nitems = static_cast<long long>(d.B) * d.X * d.Y * (d.Z / 8);
+                                 const float* b2, void* h, LiftDims d, const LiftPad* pad, int num_sms,
+                                 cudaStream_t s) {
+  const LiftPad ep = pad ? *pad : LiftPad{d.X, d.Y, d.Z, d.T};
+  const long long nitems = static_cast<long long>(d.B) * ep.X * ep.Y * (ep.Z / 8);
   const int grid = grid_for(32 * nitems, 32 * kLiftManyWarps, num_sms, 8);
   const bool regs = d.Tin == 1;
-#define DFNO_LIFT_FWD_MANY(T_, CINP_)                                                          \
-  (regs ? lift_fwd_many_launch<T_, CINP_, true>(x, W1, b1, W2, b2, h, d, grid, s)               \
-        : lift_fwd_many_launch<T_, CINP_, false>(x, W1, b1, W2, b2, h, d, grid, s))
+#define DFNO_LIFT_FWD_MANY2(T_, CINP_, P_)                                                            \
+  (regs ? lift_fwd_many_launch<T_, CINP_, true, P_>(x, W1, b1, W2, b2, h, d, ep, grid, s)              \
+        : lift_fwd_many_launch<T_, CINP_, false, P_>(x, W1, b1, W2, b2, h, d, ep, grid, s))
+#define DFNO_LIFT_FWD_MANY(T_, CINP_) (pad ? DFNO_LIFT_FWD_MANY2(T_, CINP_, true) : DFNO_LIFT_FWD_MANY2(T_, CINP_, false))
   const char* err;
   if (x_is_bf16)
     err = d.Cin <= 8 ? DFNO_LIFT_FWD_MANY(__nv_bfloat16, 8) : DFNO_LIFT_FWD_MANY(__nv_bfloat16, 16);
   else
     err = d.Cin <= 8 ? DFNO_LIFT_FWD_MANY(float, 8) : DFNO_LIFT_FWD_MANY(float, 16);
 #undef DFNO_LIFT_FWD_MANY
+#undef DFNO_LIFT_FWD_MANY2
   if (err) return err;
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
-template <typename TIn, int CINP, bool kRegs, bool kDx>
+template <typename TIn, int CINP, bool kRegs, bool kDx, bool kPad>
 static const char* lift_bwd_many_launch(const void* x, const float* W1, const float* b1, const float* W2,
                                         const float* b2, const void* dh, float* gW1, float* gb1, float* gW2,
-                                        float* gb2, float* dx, LiftDims d, int grid, cudaStream_t s) {
-  auto kern = lift_bwd_many_kernel<TIn, CINP, kRegs, kDx>;
+                                        float* gb2, float* dx, LiftDims d, LiftPad ep, int grid, cudaStream_t s) {
   static bool attr = false;                     // W1, b1 and their sums (up to 2 * kLiftMaxW floats), then x slices
-  if (const char* e = lift_many_allow_smem(kern, attr, 2 * kLiftMaxW * sizeof(float) +
-                                                           lift_many_xs_bytes<TIn>(16, kLiftMaxTin)))
-    return e;
+  const size_t most = 2 * kLiftMaxW * sizeof(float) + lift_many_xs_bytes<TIn>(16, kLiftMaxTin);
   const size_t smem = (2 * static_cast<size_t>(d.T * d.Tin + d.T) + 3) / 4 * 4 * sizeof(float) +
                       lift_many_xs_bytes<TIn>(d.Cin, d.Tin);
-  kern<<<grid, 32 * kLiftManyWarps, smem, s>>>(static_cast<const TIn*>(x), W1, b1, W2, b2, static_cast<const __nv_bfloat16*>(dh), gW1,
-                               gb1, gW2, gb2, d, dx);
+  const __nv_bfloat16* dhb = static_cast<const __nv_bfloat16*>(dh);
+  if constexpr (kPad) {
+    auto kern = lift_bwd_many_pad_kernel<TIn, CINP, kRegs, kDx>;
+    if (const char* e = lift_many_allow_smem(kern, attr, most)) return e;
+    kern<<<grid, 32 * kLiftManyWarps, smem, s>>>(static_cast<const TIn*>(x), W1, b1, W2, b2, dhb, gW1, gb1, gW2, gb2,
+                                                 d, dx, ep);
+  } else {
+    auto kern = lift_bwd_many_kernel<TIn, CINP, kRegs, kDx>;
+    if (const char* e = lift_many_allow_smem(kern, attr, most)) return e;
+    kern<<<grid, 32 * kLiftManyWarps, smem, s>>>(static_cast<const TIn*>(x), W1, b1, W2, b2, dhb, gW1, gb1, gW2, gb2,
+                                                 d, dx);
+  }
   return nullptr;
 }
 
 // 5 <= Cin <= 16: one warp per item (lift_bwd_many_kernel)
 static const char* lift_bwd_many(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
                                  const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2,
-                                 float* dx, LiftDims d, int num_sms, cudaStream_t s) {
+                                 float* dx, LiftDims d, const LiftPad* pad, int num_sms, cudaStream_t s) {
+  const LiftPad ep = pad ? *pad : LiftPad{d.X, d.Y, d.Z, d.T};
   const long long nitems = static_cast<long long>(d.B) * d.X * d.Y * (d.Z / 8);
   const int grid = grid_for(32 * nitems, 32 * kLiftManyWarps, num_sms, 8);
   const bool regs = d.Tin == 1;
+#define DFNO_LIFT_BWD_MANY4(T_, CINP_, R_, DX_, P_) \
+  lift_bwd_many_launch<T_, CINP_, R_, DX_, P_>(x, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, ep, grid, s)
 #define DFNO_LIFT_BWD_MANY3(T_, CINP_, R_, DX_) \
-  lift_bwd_many_launch<T_, CINP_, R_, DX_>(x, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, grid, s)
+  (pad ? DFNO_LIFT_BWD_MANY4(T_, CINP_, R_, DX_, true) : DFNO_LIFT_BWD_MANY4(T_, CINP_, R_, DX_, false))
 #define DFNO_LIFT_BWD_MANY2(T_, CINP_, R_) \
   (dx ? DFNO_LIFT_BWD_MANY3(T_, CINP_, R_, true) : DFNO_LIFT_BWD_MANY3(T_, CINP_, R_, false))
 #define DFNO_LIFT_BWD_MANY1(T_, CINP_) \
@@ -1060,20 +1196,29 @@ static const char* lift_bwd_many(const void* x, int x_is_bf16, const float* W1, 
 #undef DFNO_LIFT_BWD_MANY1
 #undef DFNO_LIFT_BWD_MANY2
 #undef DFNO_LIFT_BWD_MANY3
+#undef DFNO_LIFT_BWD_MANY4
   if (err) return err;
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
 const char* lift_fwd(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
-                     const float* b2, void* h, LiftDims d, int num_sms, cudaStream_t s) {
-  if (const char* e = lift_check(d)) return e;
-  if (d.Cin > 4) return lift_fwd_many(x, x_is_bf16, W1, b1, W2, b2, h, d, num_sms, s);
-  const long long nitems = static_cast<long long>(d.B) * d.X * d.Y * (d.Z / 8);
+                     const float* b2, void* h, LiftDims d, const LiftPad* pad, int num_sms, cudaStream_t s) {
+  if (const char* e = lift_check(d, pad)) return e;
+  if (d.Cin > 4) return lift_fwd_many(x, x_is_bf16, W1, b1, W2, b2, h, d, pad, num_sms, s);
+  const LiftPad ep = pad ? *pad : LiftPad{d.X, d.Y, d.Z, d.T};
+  const long long nitems = static_cast<long long>(d.B) * ep.X * ep.Y * (ep.Z / 8);
   const int grid = grid_for(nitems, 256, num_sms, 4);
   const bool regs = d.Tin == 1;
-#define DFNO_LIFT_FWD(T_, CIN_, R_) \
-  lift_fwd_kernel<T_, CIN_, R_><<<grid, 256, 0, s>>>(static_cast<const T_*>(x), W1, b1, W2, b2, static_cast<__nv_bfloat16*>(h), d)
+#define DFNO_LIFT_FWD(T_, CIN_, R_)                                                                                  \
+  do {                                                                                                               \
+    if (pad)                                                                                                         \
+      lift_fwd_pad_kernel<T_, CIN_, R_><<<grid, 256, 0, s>>>(static_cast<const T_*>(x), W1, b1, W2, b2,              \
+                                                             static_cast<__nv_bfloat16*>(h), d, ep);                 \
+    else                                                                                                             \
+      lift_fwd_kernel<T_, CIN_, R_><<<grid, 256, 0, s>>>(static_cast<const T_*>(x), W1, b1, W2, b2,                  \
+                                                         static_cast<__nv_bfloat16*>(h), d);                         \
+  } while (0)
 #define DFNO_LIFT_FWD_T(T_)                                                                         \
   switch (d.Cin) {                                                                                  \
     case 1: if (regs) DFNO_LIFT_FWD(T_, 1, true); else DFNO_LIFT_FWD(T_, 1, false); break;          \
@@ -1111,11 +1256,19 @@ const char* lift_fwd(const void* x, int x_is_bf16, const float* W1, const float*
 template <int C>
 static const char* lift_bwd_cin(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
                                 const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2,
-                                float* dx, LiftDims d, int grid, bool regs, cudaStream_t s) {
-#define DFNO_LIFT_BWD3(T_, CIN_, R_, DX_)                                                                         \
-  lift_bwd_kernel<T_, C, CIN_, R_, DX_><<<grid, 128, 0, s>>>(static_cast<const T_*>(x), W1, b1, W2, b2,           \
-                                                             static_cast<const __nv_bfloat16*>(dh), gW1, gb1, gW2, \
-                                                             gb2, d, dx)
+                                float* dx, LiftDims d, const LiftPad* pad, int grid, bool regs, cudaStream_t s) {
+  const LiftPad ep = pad ? *pad : LiftPad{d.X, d.Y, d.Z, d.T};
+#define DFNO_LIFT_BWD3(T_, CIN_, R_, DX_)                                                                            \
+  do {                                                                                                               \
+    if (pad)                                                                                                         \
+      lift_bwd_pad_kernel<T_, C, CIN_, R_, DX_><<<grid, 128, 0, s>>>(static_cast<const T_*>(x), W1, b1, W2, b2,      \
+                                                                     static_cast<const __nv_bfloat16*>(dh), gW1, gb1, \
+                                                                     gW2, gb2, d, dx, ep);                           \
+    else                                                                                                             \
+      lift_bwd_kernel<T_, C, CIN_, R_, DX_><<<grid, 128, 0, s>>>(static_cast<const T_*>(x), W1, b1, W2, b2,          \
+                                                                 static_cast<const __nv_bfloat16*>(dh), gW1, gb1,     \
+                                                                 gW2, gb2, d, dx);                                   \
+  } while (0)
 #define DFNO_LIFT_BWD2(T_, CIN_, R_) \
   if (dx) DFNO_LIFT_BWD3(T_, CIN_, R_, true); else DFNO_LIFT_BWD3(T_, CIN_, R_, false)
 #define DFNO_LIFT_BWD(CIN_)                                                                    \
@@ -1136,17 +1289,17 @@ static const char* lift_bwd_cin(const void* x, int x_is_bf16, const float* W1, c
 
 const char* lift_bwd(const void* x, int x_is_bf16, const float* W1, const float* b1, const float* W2,
                      const float* b2, const void* dh, float* gW1, float* gb1, float* gW2, float* gb2, float* dx,
-                     LiftDims d, int num_sms, cudaStream_t s) {
-  if (const char* e = lift_check(d)) return e;
+                     LiftDims d, const LiftPad* pad, int num_sms, cudaStream_t s) {
+  if (const char* e = lift_check(d, pad)) return e;
   if (dx && reinterpret_cast<uintptr_t>(dx) % 8) return "lift_bwd: dx must be 8-byte aligned";
-  if (d.Cin > 4) return lift_bwd_many(x, x_is_bf16, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, num_sms, s);
+  if (d.Cin > 4) return lift_bwd_many(x, x_is_bf16, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, pad, num_sms, s);
   const long long nitems = static_cast<long long>(d.B) * d.X * d.Y * (d.Z / 8);
   const int split = d.C > 32 ? 8 : 4;                                 // lanes per item (see lift_bwd_kernel)
   const int grid = grid_for(split * nitems, 128, num_sms, 4);
   const bool regs = d.Tin == 1;
   const char* err = nullptr;
-  DFNO_LIFT_DISPATCH_C(d.C, (err = lift_bwd_cin<kC>(x, x_is_bf16, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, grid, regs,
-                                               s)));
+  DFNO_LIFT_DISPATCH_C(d.C, (err = lift_bwd_cin<kC>(x, x_is_bf16, W1, b1, W2, b2, dh, gW1, gb1, gW2, gb2, dx, d, pad, grid,
+                                               regs, s)));
   if (err) return err;
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);

@@ -262,6 +262,13 @@ class DistributedFNO(nn.Module):
     ``backend="torch"`` forces this portable implementation.  ``input_grad=True`` asks for dL/dx on either backend
     (the fused engine refuses an input that requires grad without it).  ``out_channels`` (default 1) predicts that
     many fields from one trunk: the output is ``[B, out_channels, *spatial, T_out]``.
+
+    ``padding`` (one non-negative int per transformed axis, in the order of ``modes``) makes the Fourier layers see a
+    non-periodic field: the lifted field gets ``padding[a]`` zeros appended at the end of axis ``a``, the blocks run on
+    the larger grid (``modes`` refer to it) and the result is cropped back before the projection head (Li et al.,
+    FNO-3D).  ``None`` or all zeros is the periodic network.  The parameters do not depend on ``padding``, so a state
+    dict loads across paddings -- but the function it computes changes.  Only axes the work partition ``P_work``
+    does not split can be padded.
     """
 
     def __new__(cls, *args, backend: str = "auto", **kwargs):
@@ -275,11 +282,12 @@ class DistributedFNO(nn.Module):
                  modes: Sequence[int], num_blocks: int = 4, device=torch.device("cpu"),
                  dtype=torch.float32, plan: str = "reference", backend: str = "auto",
                  init_seed: Optional[int] = None, fft_impl: str = "torch", input_grad: bool = False,
-                 out_channels: int = 1):
+                 out_channels: int = 1, padding: Optional[Sequence[int]] = None):
         # input_grad: accepted for constructor parity with the fused engine (which returns dL/dx only when asked);
         # this backend always differentiates its input
         super().__init__()
         self.out_channels = check_out_channels(out_channels)
+        self.padding = check_padding(padding, len(in_shape) - 2)
         if init_seed is not None:       # reproducible draw (per rank; the fused engine's is partition independent)
             torch.manual_seed(int(init_seed) + 7919 * max(int(P_x.rank), 0))
         self.P_x = P_x
@@ -312,8 +320,15 @@ class DistributedFNO(nn.Module):
             self.R_out = Repartition(P_work, P_x, out_shape, dtype=dtype)
             P_x = P_work
         self.P_work = P_x
+        if self.padding is not None:
+            split = [a for a, p in enumerate(self.padding) if p and int(P_x.shape[2 + a]) > 1]
+            if split:
+                raise ValueError(f"padding {list(self.padding)} pads transformed axes {split}, which the work "
+                                 f"partition {tuple(int(s) for s in P_x.shape)} splits; only unsplit axes can be padded")
 
         self.block_in_shape = [self.in_shape[0], self.width, *self.in_shape[2:-1], self.out_timesteps]
+        if self.padding is not None:            # the blocks run on the padded grid
+            self.block_in_shape[2:] = [n + p for n, p in zip(self.block_in_shape[2:], self.padding)]
         kw = dict(device=device, dtype=dtype)
         self.linear1 = BroadcastedLinear(P_x, self.in_shape[-1], self.out_timesteps, dim=-1, **kw)
         self.linear2 = BroadcastedLinear(P_x, self.in_shape[1], self.width, dim=1, **kw)
@@ -333,8 +348,14 @@ class DistributedFNO(nn.Module):
             x = self.R_in(x)
         x = F.gelu(self.linear1(x)); dt += self.linear1.dt_comm
         x = F.gelu(self.linear2(x)); dt += self.linear2.dt_comm
+        if self.padding is not None:            # trailing zeros on every padded axis (last axis first for F.pad)
+            x = F.pad(x, [v for p in reversed(self.padding) for v in (0, p)])
         for blk in self.blocks:
             x = blk(x); dt += blk.dt_comm
+        if self.padding is not None:
+            for a, p in enumerate(self.padding):
+                if p:
+                    x = x.narrow(2 + a, 0, x.shape[2 + a] - p)
         x = F.gelu(self.linear3(x)); dt += self.linear3.dt_comm
         x = self.linear4(x); dt += self.linear4.dt_comm
         if self.R_out is not None:
@@ -348,6 +369,22 @@ def check_out_channels(out_channels) -> int:
     if isinstance(out_channels, bool) or not isinstance(out_channels, (int, np.integer)) or int(out_channels) < 1:
         raise ValueError(f"out_channels must be an integer >= 1, got {out_channels!r}")
     return int(out_channels)
+
+
+def check_padding(padding, n_axes: int) -> Optional[tuple]:
+    """``padding`` as a tuple of ``n_axes`` non-negative ints, or ``None`` when it pads nothing (``None`` or all
+    zeros); ``ValueError`` otherwise."""
+    if padding is None:
+        return None
+    if isinstance(padding, (str, bytes)) or not hasattr(padding, "__len__"):
+        raise ValueError(f"padding must be None or a sequence of {n_axes} non-negative ints, got {padding!r}")
+    if len(padding) != n_axes:
+        raise ValueError(f"padding needs one entry per transformed axis ({n_axes}), got {len(padding)}: {padding!r}")
+    for p in padding:
+        if isinstance(p, bool) or not isinstance(p, (int, np.integer)) or int(p) < 0:
+            raise ValueError(f"padding entries must be non-negative ints, got {padding!r}")
+    out = tuple(int(p) for p in padding)
+    return out if any(out) else None
 
 
 def infer_global_shape(P: Partition, local_shape: Sequence[int]) -> List[int]:

@@ -90,7 +90,7 @@ def _pencil_axis(grid: Sequence[int]) -> Optional[int]:
 def fold_onto_pencil(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, out_channels: int = 1):
     """``(P_work, R_in, R_out)``: the y-pencil over ``P_x``'s ranks and the two re-shards that move
     the network input onto it and the ``out_channels``-channel output back (``None`` when ``P_x`` already is that
-    pencil)."""
+    pencil).  Both re-shards move the unpadded tensors: a network with ``padding`` pads after its lift, on the pencil."""
     if _pencil_axis(P_x.shape) is not None:
         return P_x, None, None
     from ..parallel.primitives import Repartition
@@ -103,7 +103,7 @@ def fold_onto_pencil(P_x: Partition, in_shape: Sequence[int], out_timesteps: int
 
 
 def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width: int,
-             modes: Sequence[int], out_channels: int = 1) -> Tuple[bool, str]:
+             modes: Sequence[int], out_channels: int = 1, padding: Optional[Sequence[int]] = None) -> Tuple[bool, str]:
     """Can the fused engine run this configuration?  Returns ``(ok, reason)``.
 
     The engine computes on a ``(1,1,1,P,1,1)`` y-pencil.  Any other 6-D ``P_x`` without a batch
@@ -113,19 +113,35 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
     re-shards R1/R4 per Fourier layer (``dfno/dfno.py:247,288`` of the reference).  5-D (2-D + time)
     problems run as 6-D ones with a singleton x axis (:func:`_as_6d`).  ``out_channels`` > 1 (at most
     :data:`MAX_OUT`) runs the multi-output head kernels, which exist on the round-2 route only.  An
-    ``out_channels`` that is not an integer >= 1 raises ``ValueError``."""
-    from .fno import check_out_channels
+    ``out_channels`` that is not an integer >= 1 raises ``ValueError``.
+
+    ``padding`` (see :class:`dfno_b200.models.fno.DistributedFNO`) runs on the round-2 route only; the engine's y axis
+    (the pencil axis) can be padded at one rank only, z in multiples of 8, t by an even count.  Every other limit
+    applies to the padded extents.  Malformed ``padding`` raises ``ValueError``."""
+    from .fno import check_out_channels, check_padding
     O = check_out_channels(out_channels)
     six = _as_6d(P_x.shape, in_shape, modes)
     if six is None:
         return False, "fused engine covers 2-D + time and 3-D + time fields (5-D / 6-D tensors)"
-    grid, shape6, modes6, _ = six
+    grid, shape6, modes6, five_d = six
+    pad = check_padding(padding, len(modes))
+    pad6 = (0, 0, 0, 0) if pad is None else ((0, *pad) if five_d else pad)
     if grid[0] != 1:
         return False, "batch-partitioned P_x (data parallel) runs on the portable backend"
     P = int(np.prod(grid))
     B, Cin, X, Y, Z, Tin = shape6
     T = int(out_timesteps)
     mx, my, mz, mt = modes6
+    if pad is not None:
+        if 2 * (2 * mz) > 128:
+            return False, (f"padding {list(pad)} needs the round-2 route (2 * 2 * modes_z <= 128, here {4 * mz}); the "
+                           f"round-1 head has no padded layout")
+        if pad6[1] and P > 1:
+            return False, (f"padding {list(pad)} pads the axis the engine splits over {P} GPUs "
+                           f"({'X' if five_d else 'Y'}); only one GPU can pad it")
+        if pad6[2] % 8 or pad6[3] % 2:
+            return False, f"padding {list(pad)}: z padding must be a multiple of 8 and t padding even"
+        X, Y, Z, T = X + pad6[0], Y + pad6[1], Z + pad6[2], T + pad6[3]
     if width not in SUPPORTED_WIDTHS + WIDE_WIDTHS:
         return False, f"width {width} not in {SUPPORTED_WIDTHS} (nor in {WIDE_WIDTHS}, the round-2 widths)"
     if O > MAX_OUT:
@@ -145,7 +161,7 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
         return False, "Y and 2*modes_z must divide evenly over the pencil"
     if Cin > MAX_IN or Tin > 64:
         return False, f"lift kernels cover Cin <= {MAX_IN} and Tin <= 64"
-    lift_w = T * Tin + T + 2 * (width * Cin + width)
+    lift_w = (T - pad6[3]) * Tin + (T - pad6[3]) + 2 * (width * Cin + width)    # linear1 maps Tin -> the interior T
     if lift_w > LIFT_MAX_W:
         return False, (f"lift weights need {lift_w} floats of shared memory, more than the lift kernel's "
                        f"{LIFT_MAX_W} (kLiftMaxW)")
@@ -159,7 +175,8 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
         return False, "transformed axes: Z <= 256, T <= 128, X, Y <= 256 samples"
     if B * width * X * (Y // P) * Z * T >= 2 ** 31:
         return False, "per-rank activation must stay below 2^31 elements"
-    pl = EnginePlan(B, Cin, Tin, width, T, X, Y, Z, modes6, world=P, rank=0, out_channels=O)
+    pl = EnginePlan(B, Cin, Tin, width, T - pad6[3], X - pad6[0], Y - pad6[1], Z - pad6[2], modes6, world=P, rank=0,
+                    out_channels=O, pad=pad6)
     pl.finish(4)
     need = pl.memory_bytes(train=True)["total"]
     if need > HBM_BUDGET:
@@ -197,7 +214,7 @@ def wants(args, kwargs, backend: str) -> bool:
     dtype = cfg.get("dtype", torch.float32)
     try:
         ok, why = supports(cfg["P_x"], cfg["in_shape"], cfg["out_timesteps"], cfg["width"], cfg["modes"],
-                           out_channels=cfg.get("out_channels", 1))
+                           out_channels=cfg.get("out_channels", 1), padding=cfg.get("padding"))
     except Exception as e:           # noqa: BLE001 - malformed arguments: let the portable constructor report them
         ok, why = False, f"{type(e).__name__}: {e}"
     if backend == "fused":
@@ -216,7 +233,15 @@ def wants(args, kwargs, backend: str) -> bool:
 class EnginePlan:
     """All integer bookkeeping of one rank; no tensors, no CUDA -- unit-testable on CPU."""
 
-    def __init__(self, B, Cin, Tin, C, T, X, Y, Z, modes, world=1, rank=0, hidden=HEAD_HIDDEN, out_channels=1):
+    def __init__(self, B, Cin, Tin, C, T, X, Y, Z, modes, world=1, rank=0, hidden=HEAD_HIDDEN, out_channels=1,
+                 pad=None):
+        # pad (px, py, pz, pt): zeros appended to the lifted field.  X, Y, Z, T below are the padded extents everything
+        # between the lift and the head runs on; the network input and output keep the interior ones Xi, Yi, Zi, Ti.
+        self.pad = tuple(int(p) for p in pad) if pad else (0, 0, 0, 0)
+        self.padded = any(self.pad)
+        self.Xi, self.Yi, self.Zi, self.Ti = X, Y, Z, T
+        self.Yli = Y // world
+        X, Y, Z, T = X + self.pad[0], Y + self.pad[1], Z + self.pad[2], T + self.pad[3]
         self.B, self.Cin, self.Tin, self.C, self.T = B, Cin, Tin, C, T
         self.O = int(out_channels)                         # output channels (fields) of the head
         self.X, self.Y, self.Z = X, Y, Z
@@ -233,6 +258,7 @@ class EnginePlan:
         self.Tp = (T + 3) // 4 * 4                         # t pitch of Z1: G1b reads rows of 2*Tp bf16 (16-byte TMA pitch)
         self.BC = B * C
         self.S = X * self.Yl * T * Z                       # positions per (b, c) slab
+        self.Si = self.Xi * self.Yli * self.Ti * self.Zi   # of them interior: one output element per (b, o)
         self.npos = B * self.S
         self.Q = self.kzl * self.mt * self.KY * self.KX    # local modes
         self.CP = (C + 7) // 8 * 8                         # channels-last pitch (16-byte rows)
@@ -263,7 +289,7 @@ class EnginePlan:
             self.segments[name] = (off, tuple(shape))
             off += int(np.prod(shape))
 
-        seg("linear1.W", T, Tin); seg("linear1.b", T)
+        seg("linear1.W", self.Ti, Tin); seg("linear1.b", self.Ti)
         seg("linear2.W", C, Cin); seg("linear2.b", C)
         self.num_blocks = None
 
@@ -398,7 +424,7 @@ class EnginePlan:
             "workspaces": (max(self.n_Z1, self.n_U) + self.n_S1 + self.n_T1 + self.n_S2 + 2 * self.n_S3 + self.n_T2) * bf,
             "staging": (((self.n_S1 + self.n_T1) * bf if self.staged else 0) + self.n_small * f32
                         if self.world > 1 else 0),
-            "input_output": self.B * self.S // self.T * self.Cin * self.Tin * f32 + self.O * self.B * self.S * f32,
+            "input_output": self.B * self.Si // self.Ti * self.Cin * self.Tin * f32 + self.O * self.B * self.Si * f32,
         }
         if train and legacy:            # round-1 dataflow: channels-last head, separate bypass
             out["saved_activations"] = (2 * nb * self.n_act + nb * self.n_S3 + cl) * bf
@@ -432,7 +458,8 @@ class EnginePlan:
         legacy = not self.fused_pw
         P = self.world
         act, cl = self.n_act * bf, self.npos * self.CP * bf
-        x_in = self.B * self.S // self.T * self.Cin * self.Tin * f32    # the network input (fp32, as memory_bytes)
+        x_in = self.B * self.Si // self.Ti * self.Cin * self.Tin * f32  # the network input (fp32, as memory_bytes)
+        y_out = self.O * self.B * self.Si * f32                        # the network output
         Z1, S1, S2, S3, T2, U = (self.n_Z1 * bf, self.n_S1 * bf, self.n_S2 * bf, self.n_S3 * bf, self.n_T2 * bf,
                                  self.n_U * bf)
         T1 = self.n_T1 // self.mtp * self.mt * bf                      # valid (kt < mt) part
@@ -450,17 +477,18 @@ class EnginePlan:
             chain += [("permS1", 2 * S1, 0), ("permT1", 2 * T1, 0)]
         st = [(n, 2 * nb, b, l) for n, b, l in chain]                  # forward + adjoint chain per block
         st += [("spectral_mix fwd", nb, 2 * S3 + W, 0), ("spectral_mix bwd", nb, 3 * S3 + 2 * W, 0),
-               ("lift fwd", 1, act + x_in, 0), ("lift bwd", 1, act + x_in, 0), ("adam", 1, 7 * self.n_theta * f32, 0)]
+               ("lift fwd", 1, act + x_in, 0), ("lift bwd", 1, self.BC * self.Si * bf + x_in, 0),   # dh: interior only
+               ("adam", 1, 7 * self.n_theta * f32, 0)]
         if legacy:
             st += [("iG1a add (bwd)", nb, act, 0), ("bypass fwd", nb, 4 * act, 0), ("bypass bwd", nb, 5 * act, 0),
-                   ("head fwd", 1, cl + self.O * self.npos * f32, 0), ("head bwd", 1, 2 * cl + self.O * self.npos * f32, 0)]
+                   ("head fwd", 1, cl + y_out, 0), ("head bwd", 1, 2 * cl + y_out, 0)]
         else:
             # the chain's last GEMM also applies the bypass conv (+ GELU): reads U and the block input, writes the
             # pre-activation and the output (forward) / reads U and dpre, writes the input gradient (adjoint)
             st += [("spectral_out fwd", nb, U + 3 * act, 0), ("spectral_out adj", nb, U + 2 * act, 0),
                    ("dpre_dw", nb, 4 * act, 0),
-                   ("head fwd", 1, act + self.O * self.npos * f32, 0),
-                   ("head bwd", 1, 2 * act + 2 * self.O * self.npos * f32, 0)]
+                   ("head fwd", 1, act + y_out, 0),
+                   ("head bwd", 1, 2 * act + 2 * y_out, 0)]
         hbm = sum(c * b for _, c, b, _ in st)
         link = sum(c * l for _, c, _, l in st)
         return {"stages": st, "hbm_bytes": hbm, "nvlink_bytes": link,
@@ -581,10 +609,11 @@ class FusedDistributedFNO(nn.Module):
                  modes: Sequence[int], num_blocks: int = 4, device=torch.device("cuda"),
                  dtype=torch.bfloat16, plan: Optional[str] = None, backend: str = "fused",
                  use_p2p: Optional[bool] = None, init_seed: Optional[int] = None, input_grad: bool = False,
-                 out_channels: int = 1):
+                 out_channels: int = 1, padding: Optional[Sequence[int]] = None):
         super().__init__()
+        from .fno import check_padding
         self.input_grad = bool(input_grad)
-        ok, why = supports(P_x, in_shape, out_timesteps, width, modes, out_channels=out_channels)
+        ok, why = supports(P_x, in_shape, out_timesteps, width, modes, out_channels=out_channels, padding=padding)
         if not ok:
             raise ValueError(f"fused engine cannot run this configuration: {why}")
         from ..ops import build
@@ -601,9 +630,13 @@ class FusedDistributedFNO(nn.Module):
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
         self.dtype = torch.bfloat16
+        self.padding = check_padding(padding, len(self.modes))
         self.block_in_shape = [self.in_shape[0], self.width, *self.in_shape[2:-1], self.out_timesteps]
+        if self.padding is not None:            # the blocks run on the padded grid
+            self.block_in_shape[2:] = [n + p for n, p in zip(self.block_in_shape[2:], self.padding)]
         # 2-D + time problems run as 3-D + time with a singleton x axis (free views at entry / exit)
         _, shape6, modes6, self.five_d = _as_6d(P_x.shape, self.in_shape, self.modes)
+        pad6 = None if self.padding is None else ((0, *self.padding) if self.five_d else self.padding)
         B, Cin, X, Y, Z, Tin = shape6
         # work partition: the y-pencil the engine computes on.  A differently shaped P_x is folded
         # onto it once at the network's entry / exit (see supports()).
@@ -614,7 +647,7 @@ class FusedDistributedFNO(nn.Module):
         self.world = int(P_x.shape[pa]) if P_x.active else 1
         self.rank = int(P_x.index[pa]) if P_x.active else 0
         self.plan = EnginePlan(B, Cin, Tin, self.width, self.out_timesteps, X, Y, Z, modes6,
-                               self.world, self.rank, out_channels=self.out_channels)
+                               self.world, self.rank, out_channels=self.out_channels, pad=pad6)
         self.plan.finish(self.num_blocks)
         pl = self.plan
         self.dt_comm = 0.0
@@ -899,8 +932,13 @@ class FusedDistributedFNO(nn.Module):
     def _head_row_digits(self):
         """Row (b, x, y, t, z) of the engine layout -> element offset in the public
         ``[B, O, X, Y, Z, T]`` output: digits innermost first.  With several output channels the batch index is its
-        own digit (stride O*S) and channel o sits at + o*S (the plane stride)."""
+        own digit (stride O*S) and channel o sits at + o*S (the plane stride).  A padded plan returns a third list,
+        the interior extent of every digit (rows beyond it are padding): then z, t, y, x and b are separate digits."""
         pl = self.plan
+        if pl.padded:
+            Zi, Ti, Yli, Xi = pl.Zi, pl.Ti, pl.Yli, pl.Xi
+            return ([pl.Z, pl.T, pl.Yl, pl.X, pl.B], [Ti, 1, Zi * Ti, Yli * Zi * Ti, pl.O * pl.Si],
+                    [Zi, Ti, Yli, Xi, pl.B])
         if pl.O == 1:
             return [pl.Z, pl.T, pl.B * pl.X * pl.Yl], [pl.T, 1, pl.Z * pl.T]
         return [pl.Z, pl.T, pl.X * pl.Yl, pl.B], [pl.T, 1, pl.Z * pl.T, pl.O * pl.S]
@@ -929,15 +967,18 @@ class FusedDistributedFNO(nn.Module):
     _eval_mode = False
 
     def _lift_dims(self) -> List[int]:
+        """``[B, Cin, Tin, C, T, X, Y, Z]`` of the network input and the lifted field (+ the padded ``X, Y, Z, T`` of
+        the lift's output when the plan pads)."""
         pl = self.plan
-        return [pl.B, pl.Cin, pl.Tin, pl.C, pl.T, pl.X, pl.Yl, pl.Z]
+        dims = [pl.B, pl.Cin, pl.Tin, pl.C, pl.Ti, pl.Xi, pl.Yli, pl.Zi]
+        return dims + [pl.X, pl.Yl, pl.Z, pl.T] if pl.padded else dims
 
     def _forward(self, x: torch.Tensor, save: bool) -> torch.Tensor:
         pl, C_ = self.plan, self._C
         x = x.contiguous()
         if x.dtype not in (torch.float32, torch.bfloat16):
             x = x.float()
-        expect = (pl.B, pl.Cin, pl.X, pl.Yl, pl.Z, pl.Tin)
+        expect = (pl.B, pl.Cin, pl.Xi, pl.Yli, pl.Zi, pl.Tin)
         if self.five_d and x.dim() == 5:
             x = x.unsqueeze(2)
         if tuple(x.shape) != expect:
@@ -963,12 +1004,12 @@ class FusedDistributedFNO(nn.Module):
                                                    pre=pres[k] if save else None))
             with _nvtx("dfno.head"):
                 w3a, _ = self._head_operators_cm()
-                out = torch.empty(pl.B, pl.O, pl.X, pl.Yl, pl.Z, pl.T, device=self.device, dtype=torch.float32)
-                R, SR = self._head_row_digits()
+                out = torch.empty(pl.B, pl.O, pl.Xi, pl.Yli, pl.Zi, pl.Ti, device=self.device, dtype=torch.float32)
+                R, SR, *lim = self._head_row_digits()
                 if pl.O == 1:
-                    C_.head_fwd(hs[nb], w3a, self._w4b4(), out, pl.B, pl.C, pl.S, R, SR)
+                    C_.head_fwd(hs[nb], w3a, self._w4b4(), out, pl.B, pl.C, pl.S, R, SR, *lim)
                 else:
-                    C_.head_fwd_multi(hs[nb], w3a, self._w4b4(), out, pl.B, pl.C, pl.S, pl.O, pl.S, R, SR)
+                    C_.head_fwd_multi(hs[nb], w3a, self._w4b4(), out, pl.B, pl.C, pl.S, pl.O, pl.Si, R, SR, *lim)
                 return out.squeeze(2) if self.five_d else out
         hcl = self._saved["hcl"]
         for k in range(nb):
@@ -1020,15 +1061,15 @@ class FusedDistributedFNO(nn.Module):
             nb = self.num_blocks
             with _nvtx("dfno.head.bwd"):
                 w3a, w3t = self._head_operators_cm()
-                R, SR = self._head_row_digits()
+                R, SR, *lim = self._head_row_digits()
                 head_grads = (self._seg("linear3.W", gf), self._seg("linear3.b", gf),
                               self._seg("linear4.W", gf).view(-1), self._seg("linear4.b", gf))
                 if pl.O == 1:
                     C_.head_bwd2(hs[nb], w3a, w3t, self._seg("linear4.W").view(-1), dy.contiguous().float(),
-                                 self.ws["amax"], g, *head_grads, pl.B, pl.C, pl.S, R, SR)
+                                 self.ws["amax"], g, *head_grads, pl.B, pl.C, pl.S, R, SR, *lim)
                 else:
                     C_.head_bwd_multi(hs[nb], w3a, w3t, self._seg("linear4.W").view(-1), dy.contiguous().float(),
-                                      self.ws["amax"], g, *head_grads, pl.B, pl.C, pl.S, pl.O, pl.S, R, SR)
+                                      self.ws["amax"], g, *head_grads, pl.B, pl.C, pl.S, pl.O, pl.Si, R, SR, *lim)
             L = pl.X * pl.Yl * pl.T
             for k in reversed(range(nb)):
                 with _nvtx(f"dfno.block{k}.bwd"):
@@ -1112,7 +1153,8 @@ class FusedDistributedFNO(nn.Module):
         pl = self.plan
         return {"format": "fused-theta", "segments": dict(pl.segments), "C": pl.C, "kzl": pl.kzl, "kz_off": pl.kz_off,
                 "mt": pl.mt, "KX": pl.KX, "KY": pl.KY, "KZ": pl.KZ, "rank": self.rank, "world": self.world,
-                "num_blocks": self.num_blocks, "ndim": len(self.in_shape), "out_channels": pl.O}
+                "num_blocks": self.num_blocks, "ndim": len(self.in_shape), "out_channels": pl.O,
+                "padding": None if self.padding is None else list(self.padding)}
 
     @staticmethod
     def theta_to_canonical(theta: torch.Tensor, meta: Dict[str, object], include_pointwise: bool = True):

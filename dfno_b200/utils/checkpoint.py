@@ -163,6 +163,8 @@ def save_checkpoint(model, out_dir: str, epoch: Optional[int] = None, optimizer=
         "epoch": epoch,
         "format": "fused-theta" if _is_fused(net) else "portable",
         "engine": net.engine_meta() if _is_fused(net) else None,
+        # zeros appended to the lifted field (DistributedFNO(padding=...)); files without the entry are unpadded
+        "padding": None if getattr(net, "padding", None) is None else list(net.padding),
         # the grid the *layers* are sharded over (differs from P_x when time/channel workers were folded)
         "partition": tuple(int(s) for s in getattr(net, "P_work", P).shape),
         "world_ranks": P.world_ranks,
@@ -203,6 +205,7 @@ def load_checkpoint(model, out_dir: str, epoch: Optional[int] = None, optimizer=
             np.random.set_state(ts["rng_numpy"])
         info.update(ts["extra"])
         info["epoch"] = ts["epoch"]
+        info["padding"] = ts.get("padding")
     return info
 
 

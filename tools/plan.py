@@ -5,6 +5,7 @@ touching a GPU.
 
     python tools/plan.py --shape 128 128 128 20 --width 20 --modes 12 12 12 10 --gpus 8
     python tools/plan.py --shape 256 256 256 16 --width 32 --modes 12 12 12 8 --gpus 8 --partition 1 1 2 2 2 1
+    python tools/plan.py --shape 64 64 64 30 --width 20 --modes 8 8 8 8 --padding 0 0 0 2
 """
 import argparse
 import os
@@ -31,6 +32,8 @@ def main():
     ap.add_argument("--in-timesteps", type=int, default=1)
     ap.add_argument("--blocks", type=int, default=4)
     ap.add_argument("--out-channels", type=int, default=1, help="fields predicted by the network (default 1)")
+    ap.add_argument("--padding", type=int, nargs=4, default=None, metavar=("PX", "PY", "PZ", "PT"),
+                    help="zeros appended to the lifted field along x, y, z, t (default none)")
     ap.add_argument("--hbm-gbs", type=float, default=None,
                     help="HBM copy bandwidth for the traffic floor (default: the value measured on an H100)")
     ap.add_argument("--nvlink-gbs", type=float, default=None, help="measured peer-copy rate (default: not estimated)")
@@ -38,17 +41,19 @@ def main():
     X, Y, Z, T = a.shape
     grid = a.partition or [1, 1, 1, a.gpus, 1, 1]
     in_shape = [a.batch, a.in_channels, X, Y, Z, a.in_timesteps]
-    ok, why = supports(_Grid(grid), in_shape, T, a.width, a.modes, out_channels=a.out_channels)
+    ok, why = supports(_Grid(grid), in_shape, T, a.width, a.modes, out_channels=a.out_channels, padding=a.padding)
     print(f"P_x = {tuple(grid)}  in_shape = {in_shape}  T_out = {T}  width = {a.width}  modes = {tuple(a.modes)}"
-          + (f"  out_channels = {a.out_channels}" if a.out_channels != 1 else ""))
+          + (f"  out_channels = {a.out_channels}" if a.out_channels != 1 else "")
+          + (f"  padding = {tuple(a.padding)}" if a.padding and any(a.padding) else ""))
     print(f"fused engine: {'yes' if ok else 'no -- ' + why}")
     P = 1
     for g in grid:
         P *= g
-    if Y % P or (2 * a.modes[2]) % P:
+    pad = a.padding or (0, 0, 0, 0)
+    if (Y + pad[1]) % P or (2 * a.modes[2]) % P:
         return 0 if ok else 1
     pl = EnginePlan(a.batch, a.in_channels, a.in_timesteps, a.width, T, X, Y, Z, a.modes, world=P, rank=0,
-                    out_channels=a.out_channels)
+                    out_channels=a.out_channels, pad=pad)
     pl.finish(a.blocks)
     if tuple(grid) != (1, 1, 1, P, 1, 1):
         print(f"work partition: (1, 1, 1, {P}, 1, 1) (input / output re-sharded once per step)")
