@@ -141,6 +141,9 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
                            f"({'X' if five_d else 'Y'}); only one GPU can pad it")
         if pad6[2] % 8 or pad6[3] % 2:
             return False, f"padding {list(pad)}: z padding must be a multiple of 8 and t padding even"
+        if T == 1 and pad6[3]:
+            return False, (f"padding {list(pad)} with out_timesteps = 1: the padded t axis must be 1 or even, so a "
+                           f"single time step pads space only")
         X, Y, Z, T = X + pad6[0], Y + pad6[1], Z + pad6[2], T + pad6[3]
     if width not in SUPPORTED_WIDTHS + WIDE_WIDTHS:
         return False, f"width {width} not in {SUPPORTED_WIDTHS} (nor in {WIDE_WIDTHS}, the round-2 widths)"
@@ -166,9 +169,10 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
         return False, (f"lift weights need {lift_w} floats of shared memory, more than the lift kernel's "
                        f"{LIFT_MAX_W} (kLiftMaxW)")
     # T % 4 != 0 (e.g. the reference's two-phase run and in-module demo, T = 30) uses a padded t pitch in Z1
-    # (EnginePlan.Tp); covered by tests/test_fused_gpu.py
-    if Z % 8 or T % 2 or Y % 4 or (X % 4 and X != 1) or (mx % 2 and X != 1) or my % 2 or mz % 2:
-        return False, "extents must satisfy Z%8 = T%2 = X%4 = Y%4 = 0 and even modes (TMA pitch alignment)"
+    # (EnginePlan.Tp); covered by tests/test_fused_gpu.py.  T = 1 runs the chain without t stages (EnginePlan.has_t).
+    if Z % 8 or (T % 2 and T != 1) or Y % 4 or (X % 4 and X != 1) or (mx % 2 and X != 1) or my % 2 or mz % 2:
+        return False, ("extents must satisfy Z%8 = T%2 = X%4 = Y%4 = 0 (T = 1 or even) and even modes "
+                       "(TMA pitch alignment)")
     if (X != 1 and 2 * mx > X) or 2 * my > Y or 2 * mz > Z or mt > T // 2 + 1:
         return False, "mode counts exceed the axes"
     if max(Z, 2 * T) > 256 or max(2 * X, 2 * Y) > 512:
@@ -190,8 +194,8 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
                 continue
             try:
                 parts = pl.parts(st)
-            except ValueError as e:
-                return False, str(e)
+            except ValueError as e:      # at T = 1, G1a's columns also select the peer GPU
+                return False, str(e) + ("" if pl.has_t else " (the out_timesteps = 1 chain)")
             for _, n, _, _, _ in parts:
                 rows = 2 * n
                 if not dft_gemm_fits(rows, st["K"]):
@@ -251,10 +255,13 @@ class EnginePlan:
         self.Yl = Y // world
         self.y_off = rank * self.Yl
         self.has_x = X > 1                                 # X == 1: 2-D + time problem, no x transform (see _as_6d)
+        # T == 1 (steady problem / next-step prediction): the t-DFT and its inverse are identities on the single bin,
+        # so the chain has no G1b / iG1b, G1a scatters straight into S1 and iG2's T1 already is the last stage's input
+        self.has_t = T > 1
         self.KX, self.KY, self.KZ = (2 * self.mx if self.has_x else 1), 2 * self.my, 2 * self.mz
         self.kzl = self.KZ // world
         self.kz_off = rank * self.kzl
-        self.mtp = (self.mt + 3) // 4 * 4
+        self.mtp = (self.mt + 3) // 4 * 4 if self.has_t else 1    # kt pitch of T1 (iG1b reads 16-byte rows)
         self.Tp = (T + 3) // 4 * 4                         # t pitch of Z1: G1b reads rows of 2*Tp bf16 (16-byte TMA pitch)
         self.BC = B * C
         self.S = X * self.Yl * T * Z                       # positions per (b, c) slab
@@ -273,13 +280,14 @@ class EnginePlan:
         # element counts (bf16 unless noted)
         BC, Yl, kzl, mt, mtp = self.BC, self.Yl, self.kzl, self.mt, self.mtp
         self.n_act = BC * self.S
-        self.n_Z1 = BC * X * self.KZ * Yl * self.Tp * 2
+        # Z1 (G1a -> G1b) and U (iG1b -> last stage) exist only for the t stages: at T == 1 T1 is U's layout
+        self.n_Z1 = BC * X * self.KZ * Yl * self.Tp * 2 if self.has_t else 0
         self.n_S1 = BC * kzl * mt * X * Y * 2
         self.n_S2 = BC * kzl * mt * self.KY * X * 2
         self.n_S3 = BC * self.Q * 2
         self.n_T2 = BC * X * kzl * mt * self.KY * 2
         self.n_T1 = BC * X * Yl * self.KZ * mtp * 2
-        self.n_U = BC * X * Yl * T * self.KZ * 2
+        self.n_U = BC * X * Yl * T * self.KZ * 2 if self.has_t else 0
         # flat parameter layout (fp32 elements)
         self.segments: Dict[str, Tuple[int, Tuple[int, ...]]] = {}
         off = 0
@@ -329,7 +337,22 @@ class EnginePlan:
         m_loc = kzl * mt
         Tp = self.Tp
         st = []
-        if not staged:
+        if not self.has_t:
+            # T == 1: G1a pair-scatters the z-spectrum straight into S1 on the GPU owning kz -- the column (kz) digit
+            # picks the peer, as iG2's y does -- consecutive rows are consecutive y, the store pattern of G2
+            if not staged:      # S1[bc, kz', x, y, ri]
+                st.append(dict(name="G1a", src="src", dst="S1", M=BC * X * Yl, K=Z, lda=Z, N=2 * KZ, op="G1a",
+                               scatter=ScatterSpec(rows=[(Yl, 2), (X, Y * 2), (BC, kzl * X * Y * 2)],
+                                                   cols=(kzl, X * Y * 2, 0), peer=("col", kzl),
+                                                   base_off=self.y_off * 2),
+                               peer_dst=True, barrier_after=True))
+            else:               # S1s[bc, kz', r_src, x, y_loc, ri]
+                st.append(dict(name="G1a", src="src", dst="S1s", M=BC * X * Yl, K=Z, lda=Z, N=2 * KZ, op="G1a",
+                               scatter=ScatterSpec(rows=[(Yl, 2), (X, Yl * 2), (BC, kzl * P * X * Yl * 2)],
+                                                   cols=(kzl, P * X * Yl * 2, 0), peer=("col", kzl),
+                                                   base_off=r * X * Yl * 2),
+                               peer_dst=True, barrier_after=True))
+        elif not staged:
             st.append(dict(name="G1a", src="src", dst="Z1", M=BC * X * Yl * T, K=Z, lda=Z, N=2 * KZ, op="G1a",
                            scatter=ScatterSpec(rows=[(T, 2), (Yl, 2 * Tp), (BC * X, KZ * Yl * Tp * 2)],
                                                cols=(KZ, Yl * Tp * 2, 0))))
@@ -347,6 +370,7 @@ class EnginePlan:
                                                cols=(mt, P * X * Yl * 2, 0), peer=("row", 2, kzl),
                                                base_off=r * X * Yl * 2),
                            peer_dst=True, barrier_after=True))
+        if staged:
             # S1s[a=(bc,kzl,kt), r_src, x, y_loc] -> S1[a, x, (r_src, y_loc)]   (32-bit words = complex pairs)
             st.append(dict(name="permS1", src="S1s", dst="S1", size=[Yl, P, X, BC * m_loc],
                            sstr=[1, X * Yl, Yl, P * X * Yl], dstr=[1, Yl, Y, X * Y]))
@@ -382,10 +406,13 @@ class EnginePlan:
             st.append(dict(name="permT1", src="T1s", dst="T1", size=[mt, kzl, P, Yl, X, BC],
                            sstr=[1, mt, Yl * X * m_loc, X * m_loc, m_loc, P * Yl * X * m_loc],
                            dstr=[1, mtp, kzl * mtp, KZ * mtp, Yl * KZ * mtp, X * Yl * KZ * mtp]))
-        st.append(dict(name="iG1b", src="T1", dst="U", M=BC * X * Yl * KZ, K=2 * mt, lda=2 * mtp, N=2 * T, op="iG1b",
-                       scatter=ScatterSpec(rows=[(KZ, 2), (BC * X * Yl, T * KZ * 2)], cols=(T, KZ * 2, 0))))
-        st.append(dict(name="iG1a", src="U", dst="dst", M=BC * X * Yl * T, K=2 * KZ, lda=2 * KZ, N=Z, op="iG1a",
-                       ldc=Z))
+        if self.has_t:
+            st.append(dict(name="iG1b", src="T1", dst="U", M=BC * X * Yl * KZ, K=2 * mt, lda=2 * mtp, N=2 * T,
+                           op="iG1b",
+                           scatter=ScatterSpec(rows=[(KZ, 2), (BC * X * Yl, T * KZ * 2)], cols=(T, KZ * 2, 0))))
+        # T == 1: T1[bc, x, y_loc, kz, ri] (kt pitch 1) is U[bc, x, y_loc, t, kz, ri]
+        st.append(dict(name="iG1a", src="U" if self.has_t else "T1", dst="dst", M=BC * X * Yl * T, K=2 * KZ,
+                       lda=2 * KZ, N=Z, op="iG1a", ldc=Z))
         return st
 
     def parts(self, st: dict) -> List[Tuple[int, int, Optional[ScatterSpec], int, Optional[int]]]:
@@ -443,7 +470,8 @@ class EnginePlan:
     def cost_model(self, hbm_gbs: float = H100_COPY_GBS, nvlink_gbs: Optional[float] = None,
                    front: bool = False) -> Dict[str, object]:
         """Bytes every kernel of one training step must move (per rank) on this plan's routes and the resulting
-        floors.  ``front``: G1a + G1b run as the single ``spectral_in`` kernel (Z1 stays on the SM).
+        floors.  ``front``: G1a + G1b run as the single ``spectral_in`` kernel (Z1 stays on the SM); a T = 1 plan has
+        no G1b and ignores it.
 
         Pure bookkeeping of the dataflow in :class:`FusedDistributedFNO` -- each stage reads its input
         buffer and writes its output buffer once; nothing is assumed to stay in L2 (the working set of a
@@ -467,7 +495,10 @@ class EnginePlan:
         off = (P - 1) / P if P > 1 else 0.0
         chain = [("G1a", act + Z1, 0), ("G1b", Z1 + S1, S1 * off), ("G2", S1 + S2, 0), ("G3", S2 + S3, 0),
                  ("iG3", S3 + T2, 0), ("iG2", T2 + T1, T1 * off), ("iG1b", T1 + U, 0)]
-        if front and not legacy:
+        if not self.has_t:      # T == 1: G1a writes S1 (across NVLink), the last stage reads T1, spectral_in never runs
+            U = T1
+            chain = [("G1a", act + S1, S1 * off)] + chain[2:-1]
+        elif front and not legacy:
             chain = [("spectral_in", act + S1, S1 * off)] + chain[2:]
         if not self.has_x:
             chain = [c for c in chain if c[0] not in ("G3", "iG3")]
@@ -504,6 +535,9 @@ class EnginePlan:
             "iG1b": OPS.inv_complex_hermitian(T, self.mt), "iG1a": OPS.inv_complex_to_real(Z, self.mz),
         }
         mirror = {"G1a": "iG1a", "G1b": "iG1b", "G2": "iG2", "iG2": "G2", "iG1b": "G1b", "iG1a": "G1a"}
+        if not self.has_t:       # at T == 1 both t operators are the 2 x 2 identity: the chain has no t stages
+            for k in ("G1b", "iG1b"):
+                del f[k], mirror[k]
         if self.has_x:
             f["G3"], f["iG3"] = OPS.fwd_complex(X, self.mx), OPS.inv_complex(X, self.mx)
             mirror.update({"G3": "iG3", "iG3": "G3"})
@@ -675,13 +709,14 @@ class FusedDistributedFNO(nn.Module):
 
         # ---- workspaces
         bf = dict(device=self.device, dtype=torch.bfloat16)
-        self.ws = {
-            "Z1U": torch.empty(max(pl.n_Z1, pl.n_U), **bf),
+        # Z1 and U share one buffer; a T = 1 chain has neither
+        self.ws = {"Z1U": torch.empty(max(pl.n_Z1, pl.n_U), **bf)} if pl.has_t else {}
+        self.ws.update({
             "S1": self.sym_S1.view([pl.n_S1], torch.bfloat16) if self.world > 1 else torch.empty(pl.n_S1, **bf),
             "T1": self.sym_T1.view([pl.n_T1], torch.bfloat16) if self.world > 1 else torch.empty(pl.n_T1, **bf),
             "S2": torch.empty(pl.n_S2, **bf), "S3w": torch.empty(pl.n_S3, **bf),
             "S4": torch.empty(pl.n_S3, **bf), "T2": torch.empty(pl.n_T2, **bf),
-        }
+        })
         self._saved: Dict[str, torch.Tensor] = {}
         self._train_bufs_ready = False
         self._generation = 0                     # number of saving forwards so far (see _FusedFn)
@@ -700,8 +735,8 @@ class FusedDistributedFNO(nn.Module):
             self.ws["T1s"] = self.ws["T1"]
             self.ws["T1"] = torch.zeros(pl.n_T1, **bf)
         # the first two GEMMs of every chain (z-DFT, t-DFT) + the transpose R2 as ONE kernel that keeps Z1 on the SM
-        # (csrc/spectral_in_sm90.cu); None where spectral_in_check refuses the shape (e.g. T > 64), and then G1a + G1b
-        # run as two dft_gemm launches
+        # (csrc/spectral_in_sm90.cu); None where spectral_in_check refuses the shape (e.g. T > 64) -- then G1a + G1b
+        # run as two dft_gemm launches -- and at T = 1, whose chain has no G1b
         self.front = self._front_plan()
 
     @property
@@ -716,8 +751,10 @@ class FusedDistributedFNO(nn.Module):
 
     def _front_plan(self) -> Optional[dict]:
         """Destination view of ``spectral_in`` for this plan's S1 layout (direct or staged), or None when the kernel
-        does not support the shape (then G1a + G1b run as separate GEMMs)."""
+        does not support the shape (then G1a + G1b run as separate GEMMs) or the chain has no t stage (T = 1)."""
         pl = self.plan
+        if not pl.has_t:
+            return None
         P, r = max(self.world, 1), self.rank
         X, Y, Yl, mt, kzl = pl.X, pl.Y, pl.Yl, pl.mt, pl.kzl
         if pl.staged:        # S1s[bc, kz', kt, r_src, x, y_loc, ri] on the rank owning kz
@@ -867,9 +904,9 @@ class FusedDistributedFNO(nn.Module):
         pl = self.plan
         ws = self.ws
         s3 = self._saved["S3"][block] if (self._train_bufs_ready and not self._eval_mode) else ws["S3w"]
-        bufs = {"src": src, "Z1": ws["Z1U"], "S1": ws["S1"], "S2": ws["S2"],
+        bufs = {"src": src, "Z1": ws.get("Z1U"), "S1": ws["S1"], "S2": ws["S2"],
                 "S3": ws["S3w"] if adj else s3, "S4": ws["S4"], "T2": ws["T2"], "T1": ws["T1"],
-                "U": ws["Z1U"], "dst": dst, "S1s": ws.get("S1s"), "T1s": ws.get("T1s")}
+                "U": ws.get("Z1U"), "dst": dst, "S1s": ws.get("S1s"), "T1s": ws.get("T1s")}
         R = self._seg(f"blocks.{block}.spectral")
         for st in self.chain_desc:
             if self.front is not None and st["name"] in ("G1a", "G1b"):

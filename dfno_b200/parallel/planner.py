@@ -93,8 +93,10 @@ def validate_modes(shape: Sequence[int], modes: Sequence[int]) -> None:
                              f"got {shape[2+ax]}")
     if modes[-1] > shape[-1] // 2 + 1:
         raise ValueError(f"modes[-1]={modes[-1]} exceeds rfft bins {shape[-1]//2+1}")
-    if shape[-1] % 2:
-        raise ValueError("the last (time) axis must have even length (irfft round trip)")
+    # T = 1 (a steady problem, or next-step prediction): the single rfft bin is real-valued input, irfft(n=1) takes the
+    # real part of it back, so the block is the spatial spectral convolution with the real part taken at the end
+    if shape[-1] % 2 and shape[-1] != 1:
+        raise ValueError("the last (time) axis must have length 1 or even length (irfft round trip)")
 
 
 def spectrum_shape(block_shape: Sequence[int], modes: Sequence[int]) -> List[int]:

@@ -6,6 +6,7 @@ touching a GPU.
     python tools/plan.py --shape 128 128 128 20 --width 20 --modes 12 12 12 10 --gpus 8
     python tools/plan.py --shape 256 256 256 16 --width 32 --modes 12 12 12 8 --gpus 8 --partition 1 1 2 2 2 1
     python tools/plan.py --shape 64 64 64 30 --width 20 --modes 8 8 8 8 --padding 0 0 0 2
+    python tools/plan.py --shape 128 128 128 1 --width 20 --modes 12 12 12 1 --batch 4 --in-channels 2
 """
 import argparse
 import os
@@ -72,8 +73,9 @@ def main():
            " (no measured NVLink rate)"))
     for name, calls, hb, lb in cm["stages"]:
         print(f"  {name:18s} x{calls:<3d} {hb / 1e9:8.3f} GB/call" + (f"  + {lb / 1e6:7.1f} MB NVLink" if lb else ""))
-    print(f"\nstage chain ({'staged' if pl.staged else 'direct'} peer layout), one spectral convolution"
-          " (G1a + G1b run as ONE kernel, spectral_in, when the shape allows: T <= 64, local Y % 4 == 0):")
+    print(f"\nstage chain ({'staged' if pl.staged else 'direct'} peer layout), one spectral convolution" +
+          (" (G1a + G1b run as ONE kernel, spectral_in, when the shape allows: T <= 64, local Y % 4 == 0):"
+           if pl.has_t else " (T_out = 1: no t stages; G1a scatters into S1, the last stage reads T1):"))
     for st in pl.chain(staged=pl.staged):
         if "N" not in st:
             print(f"  {st['name']:7s} {'local permutation ' + st['src'] + ' -> ' + st['dst'] if st['name'].startswith('perm') else 'per-mode channel mixing'}")
