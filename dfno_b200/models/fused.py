@@ -622,6 +622,10 @@ class _FusedFn(torch.autograd.Function):
         if ctx.generation != eng._generation:
             raise RuntimeError("backward through a fused-engine forward whose saved activations were overwritten by a "
                                "later forward (the engine keeps one set); run forward/backward pairs back to back")
+        if getattr(ctx, "consumed", False):
+            raise RuntimeError("second backward through one fused-engine forward (retain_graph=True): the first one "
+                               "overwrote the saved pre-activations with their gradients; run the forward again")
+        ctx.consumed = True
         want_dx, want_dtheta = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         # the engine writes straight into theta.grad's storage (no 2 GB autograd copy)
         dx = eng._backward(x, dy, input_grad=want_dx, theta_grad=want_dtheta)
@@ -1067,10 +1071,11 @@ class FusedDistributedFNO(nn.Module):
 
     def _backward(self, x: torch.Tensor, dy: torch.Tensor, input_grad: bool = False,
                   theta_grad: bool = True) -> Optional[torch.Tensor]:
-        """Backward of the last saving forward.  ``theta_grad``: the weight gradients go to ``grad_flat``, which
-        becomes ``theta.grad``.  Otherwise (frozen weights) ``theta.grad`` is left as it was: the spectral-weight
-        gradients are not formed and the small segment's kernels accumulate into a scratch buffer.  ``input_grad``:
-        returns dL/dx as fp32 in the engine's local 6-D input shape (else ``None``)."""
+        """Backward of the last saving forward, at most once: it overwrites the saved pre-activations with their
+        gradients, so a second backward needs a new saving forward.  ``theta_grad``: the weight gradients go to
+        ``grad_flat``, which becomes ``theta.grad``.  Otherwise (frozen weights) ``theta.grad`` is left as it was: the
+        spectral-weight gradients are not formed and the small segment's kernels accumulate into a scratch buffer.
+        ``input_grad``: returns dL/dx as fp32 in the engine's local 6-D input shape (else ``None``)."""
         pl, C_ = self.plan, self._C
         x = x.contiguous()
         if x.dtype not in (torch.float32, torch.bfloat16):

@@ -92,17 +92,32 @@ def _run_chain(plans, ops, src, weights, adj=False, staged=False):
                                              (4, True, 8), (2, True, 8), (1, False, 6), (2, True, 6), (4, False, 6)])
 def test_stage_plan_reproduces_spectral_convolution(P, staged, max_n):
     """``max_n`` below the real limit forces the column-part path (used on the GPU for axes > 128)."""
-    import dfno_b200 as d
-    B, C, X, Y, Z, T = 2, 3, 8, (8 if max_n == 256 else 16), 8, 4
-    modes = (2, 2, 2, 3)
+    Y, T = (8 if max_n == 256 else 16), 4
     if max_n == 6:                      # T = 6 is not a multiple of 4: Z1 carries a padded t pitch (Tp = 8)
         Y, T, max_n = 8, 6, 256
+    _check_stage_plan(P, staged, 8, Y, 8, T, (2, 2, 2, 3), max_n=max_n)
+
+
+@pytest.mark.parametrize("P,staged,T,pad", [(1, False, 1, None), (2, False, 1, None), (4, False, 1, None),
+                                            (2, True, 1, None), (4, True, 1, None),
+                                            (2, False, 4, (4, 0, 8, 2)), (4, True, 4, (4, 0, 8, 2))])
+def test_stage_plan_reproduces_steady_and_padded_convolution(P, staged, T, pad):
+    """The out_timesteps = 1 chain (no t stages: G1a scatters into the owners' S1 and iG2's T1 feeds the last stage)
+    and a plan padded in x, z and t (the chain runs on the padded extents)."""
+    _check_stage_plan(P, staged, 8, 8, 8, T, (2, 2, 2, 1 if T == 1 else 2), pad=pad)
+
+
+def _check_stage_plan(P, staged, X, Y, Z, T, modes, max_n=256, pad=None):
+    """The stage plan of P ranks replayed in float64 against the portable block's spectral convolution on the
+    (padded) field, and the adjoint chain against it through <chain(x), g> = <x, chain_adj(g)>."""
+    import dfno_b200 as d
+    B, C = 2, 3
+    if pad is not None:
+        X, Y, Z, T = X + pad[0], Y + pad[1], Z + pad[2], T + pad[3]
     torch.manual_seed(0)
     _, P1, _ = d.create_standard_partitions((1, 1, 1, 1, 1, 1))
     blk = d.DistributedFNOBlock(P1, [B, C, X, Y, Z, T], modes, dtype=torch.float64)
-    state = None
     # global spectral weight [C, C, KX, KY, KZ, mt] from the block's corner parameters
-    from dfno_b200.parallel.decomposition import shard_bounds
     Wg = torch.zeros(C, C, *blk.fft_shape[2:], dtype=torch.complex128)
     for w, sl in zip(blk.weights, blk.slices):
         Wg[sl] = w.detach()
@@ -111,12 +126,19 @@ def test_stage_plan_reproduces_spectral_convolution(P, staged, max_n):
 
     plans = []
     for r in range(P):
-        pl = EnginePlan(B, 1, 1, C, T, X, Y, Z, modes, world=P, rank=r)
+        if pad is None:
+            pl = EnginePlan(B, 1, 1, C, T, X, Y, Z, modes, world=P, rank=r)
+        else:                           # interior extents + padding: the plan's X, Y, Z, T are the padded ones
+            pl = EnginePlan(B, 1, 1, C, T - pad[3], X - pad[0], Y - pad[1], Z - pad[2], modes, world=P, rank=r,
+                            pad=pad)
+            assert (pl.X, pl.Y, pl.Z, pl.T) == (X, Y, Z, T)
         pl.finish(1)
         pl.max_n = max_n
         plans.append(pl)
     if max_n != 256:
         assert sum(len(plans[0].parts(st)) > 1 for st in plans[0].chain(staged=staged) if "N" in st) == 2
+    if T == 1:
+        assert [st["name"] for st in plans[0].chain(staged=staged) if st["name"] in ("G1b", "iG1b")] == []
     ops = plans[0].operators()
     h = x.permute(0, 1, 2, 3, 5, 4).contiguous().numpy()         # engine layout [B, C, X, Y, T, Z]
     src, weights = [], []

@@ -7,7 +7,8 @@ checked:
 * the checker rejects a dx with one input channel zeroed, and a reference with one t term of the lift dropped;
 * dx does not change theta.grad, and a frozen theta (``requires_grad_(False)``) keeps theta.grad as it was while
   dx stays bitwise equal to the trainable-theta dx;
-* a double backward (``create_graph=True``) raises;
+* a double backward (``create_graph=True``) raises, and so does a second backward through one forward
+  (``retain_graph=True``), which would otherwise read gradients where the saved pre-activations were;
 * gradient descent on the input of a frozen engine (inversion) tracks the same descent on the fp32 portable backend.
 """
 import pytest
@@ -188,6 +189,21 @@ def test_double_backward_raises():
     xx = x.clone().requires_grad_()
     with pytest.raises(RuntimeError, match="double backward"):
         torch.autograd.grad((fused(xx) * w).sum(), xx, create_graph=True)
+
+
+@pytest.mark.parametrize("name", ["cin1_tin1", "large_mz"])
+def test_second_backward_through_one_forward_raises(name):
+    """The backward overwrites the saved pre-activations with their gradients (both routes), so a second backward
+    through the same forward (``retain_graph=True``) would return a wrong dx without a word; it raises instead."""
+    case = CASE[name]
+    d, ref, fused = _models(case)
+    x, w = _inputs(case, 0)
+    xx = x.clone().requires_grad_()
+    loss = (fused(xx) * w).sum()
+    (dx,) = torch.autograd.grad(loss, xx, retain_graph=True)
+    assert passes(dx, _ref_dx(ref, x, w))
+    with pytest.raises(RuntimeError, match="second backward"):
+        torch.autograd.grad(loss, xx)
 
 
 def test_default_engine_still_refuses_input_gradients():
