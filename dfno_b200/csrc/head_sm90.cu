@@ -34,10 +34,20 @@ namespace dfno {
 namespace {
 
 // ================================================================================ forward
-constexpr int kStagesHF = 6;
-constexpr int kGroupsHF = 2;                    // consumer warpgroups (kStagesHF a multiple of it: see bypass_sm90.cu)
-static_assert(kStagesHF % kGroupsHF == 0, "every ring stage must belong to one consumer warpgroup");
-constexpr int kThreadsHF = 128 * kGroupsHF + 32;
+// The epilogue is latency bound (each GELU pair is a dependent chain of about ten steps), so the warps a scheduler can
+// switch between set its speed.  KR <= 48 runs MMA1 in two 64-unit hidden halves, each followed by its share of the
+// epilogue: the accumulator is 64 registers, which lets 4 consumer warpgroups and the TMA warp share the register file
+// (17 warps, at most 120 registers each).  KR = 64, 80 keep one 128-unit pass in 2 warpgroups.
+template <int KR>
+constexpr bool kWideHF = KR > 48;
+template <int KR>
+constexpr int kGroupsHF = kWideHF<KR> ? 2 : 4;  // consumer warpgroups (kStagesHF a multiple of it: see bypass_sm90.cu)
+template <int KR>
+constexpr int kStagesHF = kWideHF<KR> ? 6 : 8;
+static_assert(kStagesHF<16> % kGroupsHF<16> == 0 && kStagesHF<80> % kGroupsHF<80> == 0,
+              "every ring stage must belong to one consumer warpgroup");
+template <int KR>
+constexpr int kThreadsHF = 128 * kGroupsHF<KR> + 32;
 
 struct HeadFwdParams {
   int B, C, KR;
@@ -55,25 +65,27 @@ template <int KR, bool kPad>
 __device__ __forceinline__ void head_fwd_body(const CUtensorMap& tmH, const CUtensorMap& tmW3, const HeadFwdParams p,
                                               const PadRowMap pm) {
   extern __shared__ __align__(1024) uint8_t smem[];
+  constexpr int kStages = kStagesHF<KR>, kGroups = kGroupsHF<KR>;
+  constexpr int kN = kWideHF<KR> ? kHidH : 64;             // hidden units per MMA1 pass
   constexpr uint32_t w3_bytes = KR > 64 ? 32768u : 16384u;  // one or two [128 hid][64] blocks
   uint8_t* s_w3 = smem;                                    // [128 hid][64] K-major block(s), column C = b3
   uint8_t* s_a = smem + w3_bytes;                          // stages x 2 halves x [KR rows][64 pos]
   constexpr uint32_t half_bytes = KR * 128;
   constexpr uint32_t stage_bytes = 2 * half_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_a + kStagesHF * stage_bytes);
-  uint64_t* full = bars;              // [6]
-  uint64_t* empty = bars + 6;         // [6]
-  uint64_t* wfull = bars + 12;
-  uint32_t* s_w4 = reinterpret_cast<uint32_t*>(bars + 14);   // [64] fp16x2 pairs of W4 (16-byte aligned)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_a + kStages * stage_bytes);
+  uint64_t* full = bars;                    // [kStages]
+  uint64_t* empty = bars + kStages;         // [kStages]
+  uint64_t* wfull = bars + 2 * kStages;
+  uint32_t* s_w4 = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 2);   // [64] fp16x2 pairs of W4 (16-byte aligned)
   float* s_b4 = reinterpret_cast<float*>(s_w4 + 64);
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const long long num_tiles = p.tiles_per_b * p.B;
 
-  for (uint32_t i = threadIdx.x; i < kStagesHF * stage_bytes / 16; i += blockDim.x)
+  for (uint32_t i = threadIdx.x; i < kStages * stage_bytes / 16; i += blockDim.x)
     reinterpret_cast<uint4*>(s_a)[i] = make_uint4(0, 0, 0, 0);
   __syncthreads();
-  for (uint32_t i = threadIdx.x; i < kStagesHF * 2 * 16; i += blockDim.x) {      // the ones row (row C) of every half
+  for (uint32_t i = threadIdx.x; i < kStages * 2 * 16; i += blockDim.x) {        // the ones row (row C) of every half
     const uint32_t hb = i >> 4, ch = i & 15;
     reinterpret_cast<uint2*>(s_a + hb * half_bytes + p.C * 128)[ch] = make_uint2(0x3F803F80u, 0x3F803F80u);
   }
@@ -82,14 +94,14 @@ __device__ __forceinline__ void head_fwd_body(const CUtensorMap& tmH, const CUte
   if (threadIdx.x == 0) s_b4[0] = p.w4b4[kHidH];
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmH); tma_prefetch_desc(&tmW3);
-    for (int s = 0; s < kStagesHF; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
     mbar_init(wfull, 1);
     fence_barrier_init();
   }
   fence_proxy_async_smem();
   __syncthreads();
 
-  if (warp == 4 * kGroupsHF) {
+  if (warp == 4 * kGroups) {
     if (lane == 0) {
       mbar_arrive_expect_tx(wfull, w3_bytes);
       tma_load_2d(s_w3, &tmW3, wfull, 0, 0);
@@ -103,7 +115,7 @@ __device__ __forceinline__ void head_fwd_body(const CUtensorMap& tmH, const CUte
         uint8_t* st = s_a + s * stage_bytes;
         tma_load_2d(st, &tmH, &full[s], p0, b * p.C);
         tma_load_2d(st + half_bytes, &tmH, &full[s], p0 + 64, b * p.C);
-        if (++s == kStagesHF) { s = 0; ph ^= 1; }
+        if (++s == kStages) { s = 0; ph ^= 1; }
       }
     }
     return;
@@ -116,46 +128,50 @@ __device__ __forceinline__ void head_fwd_body(const CUtensorMap& tmH, const CUte
 #pragma unroll
   for (int j = 0; j < 16; ++j) w4[j] = s_w4[4 * j + cq];
   mbar_wait(wfull, 0);
-  float acc[128];
+  float acc[kN];
   long long n = 0;
   for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
-    if (n % kGroupsHF != g) continue;
-    const uint32_t s = static_cast<uint32_t>(n % kStagesHF);
+    if (n % kGroups != g) continue;
+    const uint32_t s = static_cast<uint32_t>(n % kStages);
     const int b = static_cast<int>(tile / p.tiles_per_b);
     const long long pos = (tile % p.tiles_per_b) * 128 + my_row;
-    mbar_wait(&full[s], (n / kStagesHF) & 1);
+    mbar_wait(&full[s], (n / kStages) & 1);
     // pre[pos, j] = sum_c h[c, pos] W3aug[j, c]: A MN-major (positions contiguous, 64-position halves half_bytes apart)
     const uint32_t abase = smem_u32(s_a + s * stage_bytes);
-    wgmma_fence();
+    // row k of the thread: registers (kN/2)(k/2) + 4j + 2(k%2) + {0, 1} of a pass; one fp16 dot chain of 8 pairs per
+    // 64 hidden units, each chain's sum added to out[k] in hidden-unit order
+    float out[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-    for (int ks = 0; ks < KR / 16; ++ks) {
-      // k16 step ks of W3aug: 64-column block ks / 4 (a second block only at KR = 80)
-      const uint32_t w_k = KR > 64 ? (ks >> 2) * 16384 + (ks & 3) * 32 : ks * 32;
-      wg_mma128<false, 1, 0>(acc, kHidH, gdesc_mn128(abase + ks * 2048, half_bytes, 1024), half_bytes,
-                             gdesc_k128(w_addr + w_k), ks > 0 ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    acc_fence(acc);
-    if (q == 0 && lane == 0) mbar_arrive(&empty[s]);
-    // row k of the thread: registers 64(k/2) + 4j + 2(k%2) + {0, 1}; two fp16 dot chains of 8 pairs each
-    float out[4];
+    for (int hh = 0; hh < kHidH / kN; ++hh) {        // hidden units [kN hh, kN hh + kN): W3 rows 128 bytes apart
+      wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float* a = acc + 64 * (k >> 1) + 2 * (k & 1);
-      float sum = 0.f;
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        __half2 part = __float2half2_rn(0.f);
-#pragma unroll
-        for (int j = 8 * half; j < 8 * half + 8; ++j)
-          part = __hfma2(gelu_h2(h2_from_f32(a[4 * j], a[4 * j + 1])), h2_of_bits(w4[j]), part);
-        const float2 f = __half22float2(part);
-        sum += f.x + f.y;
+      for (int ks = 0; ks < KR / 16; ++ks) {
+        // k16 step ks of W3aug: 64-column block ks / 4 (a second block only at KR = 80)
+        const uint32_t w_k = KR > 64 ? (ks >> 2) * 16384 + (ks & 3) * 32 : ks * 32;
+        wg_mma128<false, 1, 0>(acc, kN, gdesc_mn128(abase + ks * 2048, half_bytes, 1024), half_bytes,
+                               gdesc_k128(w_addr + hh * kN * 128 + w_k), ks > 0 ? 1u : 0u);
       }
-      sum += __shfl_xor_sync(0xffffffffu, sum, 1);
-      sum += __shfl_xor_sync(0xffffffffu, sum, 2);
-      out[k] = sum;
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc);
+      if (hh == kHidH / kN - 1 && q == 0 && lane == 0) mbar_arrive(&empty[s]);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float* a = acc + (kN / 2) * (k >> 1) + 2 * (k & 1);
+#pragma unroll
+        for (int half = 0; half < kN / 64; ++half) {
+          __half2 part = __float2half2_rn(0.f);
+#pragma unroll
+          for (int j = 8 * half; j < 8 * half + 8; ++j)
+            part = __hfma2(gelu_h2(h2_from_f32(a[4 * j], a[4 * j + 1])), h2_of_bits(w4[(kN / 8) * hh + j]), part);
+          const float2 f = __half22float2(part);
+          out[k] += f.x + f.y;
+        }
+        if (hh == kHidH / kN - 1) {
+          out[k] += __shfl_xor_sync(0xffffffffu, out[k], 1);
+          out[k] += __shfl_xor_sync(0xffffffffu, out[k], 2);
+        }
+      }
     }
     if constexpr (kPad) {
       const long long o = pos < p.S ? pad_row_to_offset(pm, static_cast<uint32_t>(b * p.S + pos)) : -1;
@@ -167,14 +183,14 @@ __device__ __forceinline__ void head_fwd_body(const CUtensorMap& tmH, const CUte
 }
 
 template <int KR>
-__global__ void __launch_bounds__(kThreadsHF, 1)
+__global__ void __launch_bounds__(kThreadsHF<KR>, 1)
 head_fwd_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
                 const HeadFwdParams p) {
   head_fwd_body<KR, false>(tmH, tmW3, p, PadRowMap{});
 }
 
 template <int KR>
-__global__ void __launch_bounds__(kThreadsHF, 1)
+__global__ void __launch_bounds__(kThreadsHF<KR>, 1)
 head_fwd_pad_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW3,
                     const HeadFwdParams p, const __grid_constant__ PadRowMap pm) {
   head_fwd_body<KR, true>(tmH, tmW3, p, pm);
@@ -239,6 +255,7 @@ __device__ __forceinline__ void head_bwd2_body(const CUtensorMap& tmH, const CUt
   float* s_gb4 = reinterpret_cast<float*>(bars + 18);
   uint32_t* s_w4h = reinterpret_cast<uint32_t*>(bars + 20);   // [64] fp16x2 pairs of W4 (16-byte aligned)
   float* s_gw4 = reinterpret_cast<float*>(s_w4h + 64);       // [128] CTA partial sums of dW4
+  float* s_ds = s_gw4 + kHidH;                                // KR <= 48, per warpgroup: [128 positions] s dout
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const long long num_tiles = p.tiles_per_b * p.B;
@@ -382,10 +399,15 @@ __device__ __forceinline__ void head_bwd2_body(const CUtensorMap& tmH, const CUt
     } else {
       dl = pos < p.S ? p.dout[row_to_offset(p.map, static_cast<uint32_t>(b * p.S + pos))] : 0.f;
     }
-    acc_gb4 += dl;
     float dk[4];                                     // dout of the thread's rows frag_row(q, lane, k)
+    auto take_dout = [&]() {
+      acc_gb4 += dl;
+      if constexpr (!kWideHB<KR>) s_ds[128 * g + my_row] = dl * scale;   // the lanes' rows cover the tile once
 #pragma unroll
-    for (int k = 0; k < 4; ++k) dk[k] = __shfl_sync(0xffffffffu, dl, (lane & ~3) | k);
+      for (int k = 0; k < 4; ++k) dk[k] = __shfl_sync(0xffffffffu, dl, (lane & ~3) | k);
+    };
+    // KR <= 48 first uses dout after the first MMA1 half, so the load's latency hides behind the ring wait and MMA1
+    if constexpr (kWideHB<KR>) take_dout();
     mbar_wait(&a_full[s], (n / p.stages) & 1);
     const uint32_t abase = smem_u32(s_a + s * tile_bytes);
     float acc2[KR];                                  // dh0 [pos, c]: 128 x KR (KR <= 48)
@@ -437,6 +459,7 @@ __device__ __forceinline__ void head_bwd2_body(const CUtensorMap& tmH, const CUt
         wgmma_commit();
         wgmma_wait<0>();
         acc_fence(acc);
+        if (hh == 0) take_dout();
         // ---- epi A: P = W4 gelu'(pre) into the A registers and the smem tile; dW4 += dout gelu(pre)
 #pragma unroll
         for (int mh = 0; mh < 2; ++mh) {
@@ -514,27 +537,33 @@ __device__ __forceinline__ void head_bwd2_body(const CUtensorMap& tmH, const CUt
       continue;
     }
     {
-      // ---- hs: scaled fp16 copy of the h tile at the thread's rows, channels c = l%4 (mod 4); row C = the scaled
-      // gradient itself
+      // ---- hs: scaled fp16 copy of rows 0..C of the h tile, one 16-byte chunk (8 positions of one channel) per
+      // thread and step; row C = the scaled gradient itself.  Chunk pc of row r holds positions 8 (pc ^ (r % 8)).. of
+      // its 64-position half (the 128-byte swizzle); rows above C stay zero from the start.
+      asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");      // s_ds of this tile complete
       const uint8_t* src = s_a + s * tile_bytes;
+      const float* ds_t = s_ds + 128 * g;
+      const int nh = (p.C + 1) * 8;                  // chunks per half
+      for (int i = threadIdx.x & 127; i < 2 * nh; i += 128) {
+        const int mh = i >= nh ? 1 : 0, r = (i - mh * nh) >> 3, pc = i & 7;
+        const uint32_t off = mh * half_bytes + r * 128 + pc * 16;
+        const float* d = ds_t + 64 * mh + 8 * (pc ^ (r & 7));
+        const float4 d0 = *reinterpret_cast<const float4*>(d), d1 = *reinterpret_cast<const float4*>(d + 4);
+        const float dv[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+        uint32_t o[4];
+        if (r < p.C) {
+          const uint4 v = *reinterpret_cast<const uint4*>(src + off);
+          const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int row = frag_row(q, lane, k);
-        const float ds = dk[k] * scale;
-        const uint32_t colo = (row >> 6) * half_bytes + ((row & 7) << 1);
-        const uint32_t ch = (row & 63) >> 3;
+          for (int e = 0; e < 4; ++e)
+            o[e] = h2_bits(__floats2half2_rn(__uint_as_float(w[e] << 16) * dv[2 * e],
+                                             __uint_as_float(w[e] & 0xffff0000u) * dv[2 * e + 1]));
+        } else {
 #pragma unroll
-        for (int cc = 0; cc < KR / 4; ++cc) {
-          const int c = 4 * cc + cq;
-          const uint32_t off = colo + c * 128 + ((ch ^ (c & 7)) << 4);
-          if (c < p.C) {
-            const uint16_t hv = *reinterpret_cast<const uint16_t*>(src + off);
-            *reinterpret_cast<__half*>(hsbuf + off) = __float2half_rn(__uint_as_float(static_cast<uint32_t>(hv) << 16) * ds);
-          } else if (c == p.C) {
-            *reinterpret_cast<__half*>(hsbuf + off) = __float2half_rn(ds);
-          }
+          for (int e = 0; e < 4; ++e) o[e] = h2_bits(__floats2half2_rn(dv[2 * e], dv[2 * e + 1]));
         }
-    }
+        *reinterpret_cast<uint4*>(hsbuf + off) = make_uint4(o[0], o[1], o[2], o[3]);
+      }
     }
     if (leader) tma_store_wait_read();               // the previous tile's g staging is free after the barrier
     fence_proxy_async_smem();
@@ -672,15 +701,16 @@ const char* head_fwd(const void* h, const void* W3aug, const float* w4b4, float*
       return "cudaFuncSetAttribute failed";
     attr[pd][kr_i] = true;
   }
-  const uint32_t smem_bytes = (p.KR > 64 ? 32768 : 16384) + kStagesHF * 2 * p.KR * 128 + 2048 + 1024;
+  const int stages = p.KR > 48 ? kStagesHF<64> : kStagesHF<48>;
+  const uint32_t smem_bytes = (p.KR > 64 ? 32768 : 16384) + stages * 2 * p.KR * 128 + 2048 + 1024;
   const long long tiles = p.tiles_per_b * B;
   const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
 #define DFNO_HEAD_FWD(K_, ...)                                                                         \
-  if (kr_i == 0) K_<16><<<grid, kThreadsHF, smem_bytes, stream>>>(__VA_ARGS__);                          \
-  else if (kr_i == 1) K_<32><<<grid, kThreadsHF, smem_bytes, stream>>>(__VA_ARGS__);                     \
-  else if (kr_i == 2) K_<48><<<grid, kThreadsHF, smem_bytes, stream>>>(__VA_ARGS__);                     \
-  else if (kr_i == 3) K_<64><<<grid, kThreadsHF, smem_bytes, stream>>>(__VA_ARGS__);                     \
-  else K_<80><<<grid, kThreadsHF, smem_bytes, stream>>>(__VA_ARGS__);
+  if (kr_i == 0) K_<16><<<grid, kThreadsHF<16>, smem_bytes, stream>>>(__VA_ARGS__);                      \
+  else if (kr_i == 1) K_<32><<<grid, kThreadsHF<32>, smem_bytes, stream>>>(__VA_ARGS__);                 \
+  else if (kr_i == 2) K_<48><<<grid, kThreadsHF<48>, smem_bytes, stream>>>(__VA_ARGS__);                 \
+  else if (kr_i == 3) K_<64><<<grid, kThreadsHF<64>, smem_bytes, stream>>>(__VA_ARGS__);                 \
+  else K_<80><<<grid, kThreadsHF<80>, smem_bytes, stream>>>(__VA_ARGS__);
   if (pd) { DFNO_HEAD_FWD(head_fwd_pad_kernel, tmH, tmW3, p, pm) } else { DFNO_HEAD_FWD(head_fwd_kernel, tmH, tmW3, p) }
 #undef DFNO_HEAD_FWD
   cudaError_t e = cudaGetLastError();
