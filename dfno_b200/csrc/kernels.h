@@ -56,6 +56,18 @@ const char* spectral_mix_bwd(const void* x, const float* w, const void* dy, void
 const char* adam_step(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1, float beta2,
                       float eps, float weight_decay, float bias1, float bias2, float grad_scale, const float* step_dev,
                       int num_sms, cudaStream_t s);
+// the same update with its hyperparameters read from a device array (written by adam_set_hparams before every step
+// or graph replay): schedules under CUDA-graph replay, decoupled (AdamW) decay, and clipping to a global norm whose
+// sum of squares `sumsq` (nullable: no clipping) is on the device; the pre-clip norm goes to norm_out
+const char* adam_step_dev(float* p, const float* g, float* m, float* v, long long n, const double* hparams,
+                          const float* step_dev, float grad_scale, const double* sumsq, float* norm_out, int num_sms,
+                          cudaStream_t s);
+const char* adam_set_hparams(double* hparams, double lr, double beta1, double beta2, double eps, double weight_decay,
+                             bool decoupled, double max_norm, cudaStream_t s);
+// out[0] = sum(x*x) over n fp32 values, in fp64, deterministic (fixed grid and reduction order); partials holds
+// max_blocks doubles, ticket one zeroed uint32 that the kernel leaves at zero
+const char* sumsq(const float* x, long long n, double* out, double* partials, int max_blocks, unsigned* ticket,
+                  int num_sms, cudaStream_t s);
 
 // cross-GPU flag barrier over NVLink-mapped signal pads: every rank bumps its slot on each
 // peer to `epoch`, then waits until all of its own slots reached `epoch`.
@@ -65,6 +77,8 @@ const char* p2p_barrier(uint32_t* const* peer_flags, uint32_t* my_flags, int ran
 // sum-all-reduce of a small fp32 vector through peer reads (every rank reads all peers' copies)
 const char* p2p_allreduce_small(float* const* peer_bufs, float* out, long long n, int rank, int world,
                                 cudaStream_t s);
+// out = sum over ranks, in rank order, of the fp64 scalar at each peer pointer
+const char* p2p_sum_f64(double* const* peer_bufs, double* out, int world, cudaStream_t s);
 
 // push all-to-all-v over peer memory: segment i of `send` ([send_off[i], send_off[i+1]) bytes) is stored at
 // byte offset dst_off[i] of peer i's receive buffer.  Follow with p2p_barrier before reading.

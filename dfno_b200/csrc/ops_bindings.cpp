@@ -133,6 +133,53 @@ void adam_step(at::Tensor& p, const at::Tensor& g, at::Tensor& m, at::Tensor& v,
         "adam_step");
 }
 
+double* dptr_mut(at::Tensor& t) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kDouble && t.is_contiguous(), "expected contiguous CUDA fp64 tensor");
+  return t.data_ptr<double>();
+}
+
+void adam_step_dev(at::Tensor& p, const at::Tensor& g, at::Tensor& m, at::Tensor& v, at::Tensor& hparams,
+                   const at::Tensor& step_dev, double grad_scale, const c10::optional<at::Tensor>& sumsq,
+                   const c10::optional<at::Tensor>& norm_out) {
+  TORCH_CHECK(p.numel() == g.numel() && p.numel() == m.numel() && p.numel() == v.numel(), "adam: size mismatch");
+  TORCH_CHECK(hparams.numel() >= 8 && step_dev.numel() >= 1, "adam: hparams holds 8 doubles, step_dev one float");
+  TORCH_CHECK(sumsq.has_value() == norm_out.has_value(), "adam: sumsq and norm_out go together");
+  TORCH_CHECK(!sumsq || sumsq->numel() >= 1, "adam: empty sumsq");
+  c10::cuda::CUDAGuard guard(p.device());
+  at::Tensor sq = sumsq ? *sumsq : at::Tensor(), nrm = norm_out ? *norm_out : at::Tensor();
+  check(dfno::adam_step_dev(fptr_mut(p), fptr(g), fptr_mut(m), fptr_mut(v), p.numel(), dptr_mut(hparams),
+                            fptr(step_dev), static_cast<float>(grad_scale), sumsq ? dptr_mut(sq) : nullptr,
+                            norm_out ? fptr_mut(nrm) : nullptr, sm_count(), cur_stream()),
+        "adam_step_dev");
+}
+
+void adam_set_hparams(at::Tensor& hparams, double lr, double beta1, double beta2, double eps, double weight_decay,
+                      bool decoupled, double max_norm) {
+  TORCH_CHECK(hparams.numel() >= 8, "adam: hparams holds 8 doubles");
+  c10::cuda::CUDAGuard guard(hparams.device());
+  check(dfno::adam_set_hparams(dptr_mut(hparams), lr, beta1, beta2, eps, weight_decay, decoupled, max_norm,
+                               cur_stream()), "adam_set_hparams");
+}
+
+void sumsq(const at::Tensor& x, at::Tensor& out, at::Tensor& partials, at::Tensor& ticket) {
+  TORCH_CHECK(x.dim() == 1, "sumsq: x must be a 1-D fp32 vector");
+  TORCH_CHECK(out.numel() >= 1, "sumsq: empty out");
+  TORCH_CHECK(ticket.is_cuda() && ticket.scalar_type() == at::kInt && ticket.numel() >= 1, "sumsq: int32 ticket");
+  TORCH_CHECK(partials.numel() >= 1, "sumsq: partials needs room for at least one block");
+  c10::cuda::CUDAGuard guard(x.device());
+  check(dfno::sumsq(fptr(x), x.numel(), dptr_mut(out), dptr_mut(partials), static_cast<int>(partials.numel()),
+                    reinterpret_cast<unsigned*>(ticket.data_ptr<int>()), sm_count(), cur_stream()), "sumsq");
+}
+
+void p2p_sum_f64(const std::vector<int64_t>& buf_ptrs, at::Tensor& out) {
+  const int world = static_cast<int>(buf_ptrs.size());
+  TORCH_CHECK(world >= 1 && world <= 8, "p2p_sum_f64: 1..8 peer pointers");
+  TORCH_CHECK(out.numel() >= 1, "p2p_sum_f64: empty out");
+  double* peers[8];
+  for (int i = 0; i < 8; ++i) peers[i] = reinterpret_cast<double*>(buf_ptrs[i < world ? i : 0]);
+  check(dfno::p2p_sum_f64(peers, dptr_mut(out), world, cur_stream()), "p2p_sum_f64");
+}
+
 void p2p_barrier(const std::vector<int64_t>& flag_ptrs, int64_t rank, int64_t epoch, double timeout_s) {
   const int world = static_cast<int>(flag_ptrs.size());
   uint32_t* peers[8];
@@ -425,6 +472,12 @@ void register_ops(pybind11::module& m) {
   m.def("adam_step", &adam_step, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("lr"), py::arg("beta1"),
         py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"), py::arg("grad_scale"),
         py::arg("step_dev") = c10::nullopt);
+  m.def("adam_step_dev", &adam_step_dev, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("hparams"),
+        py::arg("step_dev"), py::arg("grad_scale"), py::arg("sumsq") = c10::nullopt, py::arg("norm_out") = c10::nullopt);
+  m.def("adam_set_hparams", &adam_set_hparams, py::arg("hparams"), py::arg("lr"), py::arg("beta1"), py::arg("beta2"),
+        py::arg("eps"), py::arg("weight_decay"), py::arg("decoupled"), py::arg("max_norm"));
+  m.def("sumsq", &sumsq, py::arg("x"), py::arg("out"), py::arg("partials"), py::arg("ticket"));
+  m.def("p2p_sum_f64", &p2p_sum_f64);
   m.def("p2p_barrier", &p2p_barrier);
   m.def("p2p_allreduce_small", &p2p_allreduce_small);
   m.def("p2p_alltoall", &p2p_alltoall);

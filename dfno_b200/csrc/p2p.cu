@@ -16,6 +16,8 @@
 //                        the gradient reduction of the replicated pointwise weights -- the
 //                        Broadcast/SumReduce pair of the reference's BroadcastedLinear
 //                        (SURVEY.md K1, K18) collapses to one such call per optimizer step.
+//   p2p_sum_f64        : the same for one fp64 scalar per rank (each rank's part of the squared
+//                        gradient norm): a fixed rank order, so every rank gets the same bits.
 #include "sm90_ptx.cuh"
 #include "kernels.h"
 
@@ -24,6 +26,7 @@ namespace {
 
 struct PeerFlags { uint32_t* p[8]; };
 struct PeerBufs { const float* p[8]; };
+struct PeerF64 { const double* p[8]; };
 
 __device__ __forceinline__ unsigned long long global_timer_ns() {
   unsigned long long t;
@@ -71,6 +74,14 @@ p2p_allreduce_kernel(PeerBufs bufs, float* __restrict__ out, long long n, int wo
     float acc = 0.f;
     for (int r = 0; r < world; ++r) acc += bufs.p[r][i];
     out[i] = acc;
+  }
+}
+
+__global__ void p2p_sum_f64_kernel(PeerF64 bufs, double* __restrict__ out, int world) {
+  if (threadIdx.x == 0) {
+    double acc = 0.0;
+    for (int r = 0; r < world; ++r) acc += bufs.p[r][0];
+    *out = acc;
   }
 }
 
@@ -146,6 +157,15 @@ const char* p2p_allreduce_small(float* const* peer_bufs, float* out, long long n
   if (blocks > 64) blocks = 64;
   if (blocks < 1) blocks = 1;
   p2p_allreduce_kernel<<<static_cast<int>(blocks), 256, 0, s>>>(pb, out, n, world);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
+const char* p2p_sum_f64(double* const* peer_bufs, double* out, int world, cudaStream_t s) {
+  if (world < 1 || world > 8) return "p2p_sum_f64: world size must be 1..8";
+  PeerF64 pb;
+  for (int i = 0; i < 8; ++i) pb.p[i] = peer_bufs[i < world ? i : 0];
+  p2p_sum_f64_kernel<<<1, 32, 0, s>>>(pb, out, world);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }

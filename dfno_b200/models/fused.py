@@ -1286,19 +1286,123 @@ class FusedDistributedFNO(nn.Module):
 # optimizer
 # =====================================================================================
 
-class FusedAdam:
-    """Adam on the engine's flat parameter buffer with one fused kernel launch per step
-    (``csrc/optim.cu``); semantics of ``torch.optim.Adam`` (L2 ``weight_decay``)."""
+SUMSQ_MAX_BLOCKS = 2048          # partials of the gradient sum-of-squares kernel
+
+
+class FusedAdam(torch.optim.Optimizer):
+    """Adam on the engine's flat parameter buffer with one fused kernel launch per step (``csrc/optim.cu``):
+    ``torch.optim.Adam(..., decoupled_weight_decay=...)`` on one parameter group holding ``model.theta``, after
+    ``torch.nn.utils.clip_grad_norm_(params, max_grad_norm)`` when that is set.
+
+    ``lr``, ``betas``, ``eps`` and ``weight_decay`` are attributes that map to ``param_groups[0]``, so
+    ``torch.optim.lr_scheduler`` schedulers work on it.  Two paths:
+
+    * the defaults (no clipping, L2 decay, no scheduler attached): the hyperparameters are kernel arguments.  A captured
+      CUDA graph bakes them in; :class:`~dfno_b200.trainer.Trainer` recaptures when they change.
+    * otherwise: the kernel reads them from a device array that :meth:`write_hparams` fills before every eager step
+      and, under CUDA-graph replay, before every replay -- so replay ``k`` uses the values set before replay ``k``,
+      with no host synchronisation.  ``max_grad_norm`` adds one read of the gradient: its global sum of squares (over
+      every rank's spectral shard, the replicated pointwise segment counted once) reduced on the device.  The pre-clip
+      norm, ``clip_grad_norm_``'s return value, is the device tensor :attr:`grad_norm`.  ``max_grad_norm=inf`` measures
+      the norm without clipping.
+
+    Non-finite norms behave as in ``clip_grad_norm_(error_if_nonfinite=False)``: an infinite norm scales the gradient
+    by 0 (infinite entries become NaN), a NaN norm makes it NaN.  Nothing skips a step."""
 
     def __init__(self, model: FusedDistributedFNO, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
-                 weight_decay: float = 0.0):
+                 weight_decay: float = 0.0, decoupled_weight_decay: bool = False,
+                 max_grad_norm: Optional[float] = None):
+        betas = tuple(float(b) for b in betas)
+        if not 0.0 <= lr:
+            raise ValueError(f"invalid learning rate: {lr}")
+        if not 0.0 <= eps:
+            raise ValueError(f"invalid epsilon value: {eps}")
+        if len(betas) != 2 or not all(0.0 <= b < 1.0 for b in betas):
+            raise ValueError(f"invalid betas: {betas} (two values in [0, 1))")
+        if not 0.0 <= weight_decay:
+            raise ValueError(f"invalid weight_decay value: {weight_decay}")
+        self._check_max_grad_norm(max_grad_norm)
         self.model = model
-        self.lr, self.betas, self.eps, self.weight_decay = lr, betas, eps, weight_decay
-        self.m = torch.zeros_like(model.theta.data)
-        self.v = torch.zeros_like(model.theta.data)
+        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
+                        decoupled_weight_decay=bool(decoupled_weight_decay), max_grad_norm=max_grad_norm)
+        super().__init__([model.theta], defaults)
+        theta = model.theta.data
+        self.m = torch.zeros_like(theta)
+        self.v = torch.zeros_like(theta)
         self.step_count = 0
         # the step counter also lives on the device so a captured CUDA graph can replay the update
-        self.step_dev = torch.zeros(1, device=model.theta.device, dtype=torch.float32)
+        self.step_dev = torch.zeros(1, device=theta.device, dtype=torch.float32)
+        self.hparams = torch.zeros(8, device=theta.device, dtype=torch.float64)      # see write_hparams
+        self.grad_norm: Optional[torch.Tensor] = None
+        self._sumsq = None                                                            # (total, partials, ticket)
+        self._device_hparams = False                                                  # see use_device_hparams
+
+    @staticmethod
+    def _check_max_grad_norm(v) -> None:
+        if v is not None and not float(v) > 0.0:
+            raise ValueError(f"invalid max_grad_norm: {v} (None, or a positive value; inf measures without clipping)")
+
+    def add_param_group(self, param_group) -> None:
+        if self.param_groups:
+            raise ValueError("FusedAdam has one parameter group, the engine's flat theta")
+        super().add_param_group(param_group)
+
+    # the hyperparameters live in the param group (where schedulers change them)
+    def _group_attr(name):                                                      # noqa: N805 - property factory
+        return property(lambda self: self.param_groups[0][name],
+                        lambda self, v: self.param_groups[0].__setitem__(name, v))
+
+    lr = _group_attr("lr")
+    betas = _group_attr("betas")
+    eps = _group_attr("eps")
+    weight_decay = _group_attr("weight_decay")
+    decoupled_weight_decay = _group_attr("decoupled_weight_decay")
+    del _group_attr
+
+    @property
+    def max_grad_norm(self) -> Optional[float]:
+        return self.param_groups[0]["max_grad_norm"]
+
+    @max_grad_norm.setter
+    def max_grad_norm(self, v) -> None:
+        self._check_max_grad_norm(v)
+        self.param_groups[0]["max_grad_norm"] = v
+
+    def device_hparams(self) -> bool:
+        """Whether the step reads its hyperparameters from the device (clipping, decoupled decay, a scheduler --
+        which leaves ``initial_lr`` in the group -- attached, or :meth:`use_device_hparams`)."""
+        g = self.param_groups[0]
+        return (self._device_hparams or bool(g["decoupled_weight_decay"]) or g["max_grad_norm"] is not None
+                or "initial_lr" in g)
+
+    def use_device_hparams(self) -> None:
+        """Read the hyperparameters from the device from now on, also with the defaults.  The Trainer calls this when
+        lr, betas, eps or weight_decay change under a graph captured on the host-argument path, so that it captures
+        once more instead of on every change."""
+        self._device_hparams = True
+
+    def graph_key(self):
+        """What a CUDA graph captured around :meth:`step` depends on: a graph captured under another key must be
+        captured again."""
+        g = self.param_groups[0]
+        if self.device_hparams():
+            return ("device", g["max_grad_norm"] is not None)
+        return ("host", float(g["lr"]), tuple(g["betas"]), float(g["eps"]), float(g["weight_decay"]))
+
+    def write_hparams(self) -> None:
+        """Copy the param group's hyperparameters into the device array the step reads (one small kernel, its values
+        passed as arguments: no host synchronisation).  :meth:`step` calls it unless the stream is capturing; call it
+        before each replay of a graph that holds the step (the Trainer does)."""
+        g = self.param_groups[0]
+        b1, b2 = g["betas"]
+        mx = g["max_grad_norm"]
+        self.model._C.adam_set_hparams(self.hparams, float(g["lr"]), float(b1), float(b2), float(g["eps"]),
+                                       float(g["weight_decay"]), bool(g["decoupled_weight_decay"]),
+                                       math.inf if mx is None else float(mx))
+
+    def before_replay(self) -> None:
+        if self.device_hparams():
+            self.write_hparams()
 
     def zero_grad(self, set_to_none: bool = True) -> None:
         if set_to_none:
@@ -1306,22 +1410,77 @@ class FusedAdam:
         elif self.model.theta.grad is not None:
             self.model.theta.grad.zero_()
 
-    def step(self, grad_scale: float = 1.0) -> None:
+    @torch.no_grad()
+    def step(self, closure=None, grad_scale: float = 1.0):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
         g = self.model.theta.grad
         if g is None:
-            return
+            return loss
         self.step_count += 1
         self.step_dev += 1.0
-        self.model._C.adam_step(self.model.theta.data, g.contiguous(), self.m, self.v, self.lr, self.betas[0],
-                                self.betas[1], self.eps, self.weight_decay, self.step_count, grad_scale,
-                                self.step_dev)
+        C_ = self.model._C
+        if not self.device_hparams():
+            C_.adam_step(self.model.theta.data, g.contiguous(), self.m, self.v, self.lr, self.betas[0],
+                         self.betas[1], self.eps, self.weight_decay, self.step_count, grad_scale, self.step_dev)
+            return loss
+        if not torch.cuda.is_current_stream_capturing():
+            self.write_hparams()
+        g = g.contiguous()
+        sq = None
+        if self.max_grad_norm is not None:
+            if self.grad_norm is None:
+                self.grad_norm = torch.full((), math.nan, device=g.device, dtype=torch.float32)
+            sq = self._global_sumsq(g)
+        C_.adam_step_dev(self.model.theta.data, g, self.m, self.v, self.hparams, self.step_dev, grad_scale, sq,
+                         self.grad_norm if sq is not None else None)
+        return loss
+
+    def _global_sumsq(self, g: torch.Tensor) -> torch.Tensor:
+        """Sum of squares of the whole network's gradient, the same on every rank, as a device fp64 scalar.  The
+        replicated pointwise segment ``[0, n_small)`` is bitwise the same on every rank after the backward's
+        all-reduce, so only rank 0 counts it; each rank's spectral shard is summed across the pencil through peer
+        memory (no NCCL)."""
+        mdl, C_ = self.model, self.model._C
+        if self._sumsq is None:
+            dev = g.device
+            self._sumsq = (torch.zeros(1, device=dev, dtype=torch.float64),
+                           torch.zeros(SUMSQ_MAX_BLOCKS, device=dev, dtype=torch.float64),
+                           torch.zeros(1, device=dev, dtype=torch.int32))
+        total, partials, ticket = self._sumsq
+        flat = g.view(-1)
+        if getattr(mdl, "world", 1) <= 1:
+            C_.sumsq(flat, total, partials, ticket)
+            return total
+        mine = flat if mdl.rank == 0 else flat[mdl.plan.n_small:]
+        if mdl.use_p2p:
+            stage = mdl.sym_small.view([1], torch.float64)
+            mdl.barrier()                        # earlier readers of the staging buffer are done
+            C_.sumsq(mine, stage, partials, ticket)
+            mdl.barrier()                        # every rank's part is visible
+            C_.p2p_sum_f64(mdl.sym_small.peer_ptrs(), total)
+        else:
+            C_.sumsq(mine, total, partials, ticket)
+            dist.all_reduce(total, group=mdl.P_work.group)
+        return total
 
     def state_dict(self):
+        group = {k: v for k, v in self.param_groups[0].items() if k != "params"}
         return {"m": self.m, "v": self.v, "step": self.step_count, "lr": self.lr, "betas": self.betas,
-                "eps": self.eps, "weight_decay": self.weight_decay}
+                "eps": self.eps, "weight_decay": self.weight_decay,
+                "decoupled_weight_decay": self.decoupled_weight_decay, "max_grad_norm": self.max_grad_norm,
+                "param_group": group}
 
     def load_state_dict(self, sd) -> None:
+        """Also takes the state dicts written before decoupled decay and clipping existed: plain Adam, no clipping."""
         self.m.copy_(sd["m"]); self.v.copy_(sd["v"])
         self.step_count = int(sd["step"])
         self.step_dev.fill_(float(self.step_count))
+        group = self.param_groups[0]
+        if "param_group" in sd:                  # scheduler entries (initial_lr, ...) too
+            group.update({k: v for k, v in sd["param_group"].items() if k != "params"})
         self.lr, self.betas, self.eps, self.weight_decay = sd["lr"], tuple(sd["betas"]), sd["eps"], sd["weight_decay"]
+        self.decoupled_weight_decay = bool(sd.get("decoupled_weight_decay", False))
+        self.max_grad_norm = sd.get("max_grad_norm")

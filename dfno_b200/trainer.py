@@ -7,7 +7,7 @@ computes; the loss value is read back from a pinned scalar.
 """
 from __future__ import annotations
 
-from typing import Optional, Tuple
+from typing import Callable, Optional, Tuple
 
 import torch
 
@@ -16,8 +16,12 @@ __all__ = ["Trainer", "InferenceSession"]
 
 class Trainer:
     def __init__(self, model, criterion, optimizer, device: Optional[torch.device] = None,
-                 target_dtype: Optional[torch.dtype] = None, cuda_graph: bool = False):
+                 target_dtype: Optional[torch.dtype] = None, cuda_graph: bool = False,
+                 before_step: Optional[Callable[[], None]] = None):
+        """``before_step``: called between the backward and ``optimizer.step()``, e.g. gradient clipping for a
+        ``torch.optim`` optimizer (:class:`FusedAdam` clips inside its step: ``max_grad_norm``)."""
         self.model, self.criterion, self.optimizer = model, criterion, optimizer
+        self.before_step = before_step
         self.device = torch.device(device) if device is not None else next(model.parameters()).device
         self.cuda = self.device.type == "cuda"
         self.copy_stream = torch.cuda.Stream(device=self.device) if self.cuda else None
@@ -33,6 +37,7 @@ class Trainer:
         # step instead of a few hundred.  Falls back to eager execution if capture is not possible.
         self.cuda_graph = bool(cuda_graph) and self.cuda
         self._graph = None
+        self._graph_key = None
         self._graph_failed = False
         self.graph_kernel_launches = 0
 
@@ -94,10 +99,21 @@ class Trainer:
         y_hat = self.model(xd)
         loss = self.criterion(y_hat, yd)
         loss.backward()
+        if self.before_step is not None:
+            self.before_step()
         self.optimizer.step()
         return loss
 
     def _graphed(self, xd: torch.Tensor, yd: torch.Tensor) -> torch.Tensor:
+        opt = self.optimizer
+        key = opt.graph_key() if hasattr(opt, "graph_key") else None
+        if self._graph is not None and key != self._graph_key:
+            # the captured step baked in other hyperparameters: capture again, on the device-hyperparameter path so
+            # that later changes need no further capture
+            if key[0] == "host" and hasattr(opt, "use_device_hparams"):
+                opt.use_device_hparams()
+                key = opt.graph_key()
+            self._graph = None
         if self._graph is None:
             try:
                 self._gx, self._gy = torch.empty_like(xd), torch.empty_like(yd)
@@ -120,7 +136,7 @@ class Trainer:
                     self._gloss = self._eager(self._gx, self._gy).detach()
                 self.graph_kernel_launches = getattr(counter, "count", 0) - c0
                 self._restore_training_state(snap)
-                self._graph = graph
+                self._graph, self._graph_key = graph, key
                 self._graph_steps_py = getattr(self.optimizer, "step_count", None)
             except Exception as e:                            # noqa: BLE001 - capture is an optimisation
                 import warnings
@@ -131,9 +147,14 @@ class Trainer:
                 return self._eager(xd, yd)
         self._gx.copy_(xd, non_blocking=True)
         self._gy.copy_(yd, non_blocking=True)
+        if hasattr(opt, "before_replay"):
+            opt.before_replay()                               # this replay's lr, betas, ... into the device scalars
         self._graph.replay()
-        if hasattr(self.optimizer, "step_count"):
-            self.optimizer.step_count += 1                    # host mirror of the device-side counter
+        if hasattr(opt, "step_count"):
+            opt.step_count += 1                               # host mirror of the device-side counter
+        # what the step wrapper of an attached lr scheduler records on an eager step (else scheduler.step() warns
+        # that it ran before optimizer.step())
+        opt._opt_called = True
         counter = getattr(self.model, "_C", None)
         if hasattr(counter, "count"):
             counter.count += self.graph_kernel_launches

@@ -147,8 +147,9 @@ def checkpoint_path(out_dir: str, rank: int, epoch: Optional[int] = None, kind: 
 
 
 def save_checkpoint(model, out_dir: str, epoch: Optional[int] = None, optimizer=None,
-                    extra: Optional[Dict[str, Any]] = None, P: Optional[Partition] = None) -> str:
-    """Write this rank's files.  Returns the model file path."""
+                    extra: Optional[Dict[str, Any]] = None, P: Optional[Partition] = None, scheduler=None) -> str:
+    """Write this rank's files (with the optimizer's and an lr scheduler's state when given).  Returns the model
+    file path."""
     net = _unwrap(model)
     P = P or net.P_x
     if not P.active:                # a world rank outside P_x owns nothing: it must not clobber rank 0's files
@@ -169,6 +170,7 @@ def save_checkpoint(model, out_dir: str, epoch: Optional[int] = None, optimizer=
         "partition": tuple(int(s) for s in getattr(net, "P_work", P).shape),
         "world_ranks": P.world_ranks,
         "optimizer": optimizer.state_dict() if optimizer is not None else None,
+        "scheduler": scheduler.state_dict() if scheduler is not None else None,
         "rng_cpu": torch.get_rng_state(),
         "rng_cuda": torch.cuda.get_rng_state() if torch.cuda.is_available() else None,
         "rng_numpy": np.random.get_state(),
@@ -179,7 +181,8 @@ def save_checkpoint(model, out_dir: str, epoch: Optional[int] = None, optimizer=
 
 
 def load_checkpoint(model, out_dir: str, epoch: Optional[int] = None, optimizer=None,
-                    restore_rng: bool = True, map_location=None, P: Optional[Partition] = None) -> Dict[str, Any]:
+                    restore_rng: bool = True, map_location=None, P: Optional[Partition] = None,
+                    scheduler=None) -> Dict[str, Any]:
     """Load this rank's files (same partition as at save time).  Returns the ``extra`` dict
     plus ``epoch``."""
     net = _unwrap(model)
@@ -198,6 +201,8 @@ def load_checkpoint(model, out_dir: str, epoch: Optional[int] = None, optimizer=
                              f"model uses {tuple(P.shape)}; use reshard_checkpoint()")
         if optimizer is not None and ts["optimizer"] is not None:
             optimizer.load_state_dict(ts["optimizer"])
+        if scheduler is not None and ts.get("scheduler") is not None:
+            scheduler.load_state_dict(ts["scheduler"])
         if restore_rng:
             torch.set_rng_state(ts["rng_cpu"])
             if ts["rng_cuda"] is not None and torch.cuda.is_available():

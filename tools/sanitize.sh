@@ -12,6 +12,10 @@ $CS python -m pytest tests/test_dft_gemm_gpu.py tests/test_fused_pointwise_gpu.p
     tests/test_spectral_in_gpu.py -x -q -k "rowmajor or scatter or spectral_out or dpre_dw or head or forward_inverse or spectral_in" \
     > sanitize_logs/sanitize_${tool}.log 2>&1 || rc=$?
 tail -n 5 sanitize_logs/sanitize_${tool}.log
+# the optimizer kernels: sum of squares, both Adam paths, the replayed step
+$CS python -m pytest tests/test_fused_optim_gpu.py -x -q -k "sumsq or nonfinite or (matches_torch and step) or no_host_sync" \
+    > sanitize_logs/sanitize_${tool}_optim.log 2>&1 || rc=$?
+tail -n 5 sanitize_logs/sanitize_${tool}_optim.log
 if [ "${N:-1}" -ge 2 ]; then
   DFNO_TEST_WORLD=2 $CS python -m pytest tests/test_fused_multigpu.py tests/test_p2p_multigpu.py -x -q \
       > sanitize_logs/sanitize_${tool}_2gpu.log 2>&1 || rc=$?

@@ -46,6 +46,7 @@ ap.add_argument("--generate-visualization", "-gv", action="store_true")
 ap.add_argument("--out-root", type=Path, default=Path("data"))
 ap.add_argument("--dtype", default="auto", choices=["auto", "bf16", "fp32"],
                 help="auto: bf16 on a GPU (the fused sm_90a engine serves 2-D + time problems), fp32 on the CPU")
+d.add_optimizer_args(ap)
 args = ap.parse_args()
 
 d.ensure_process_group()
@@ -100,10 +101,8 @@ with ctx:
                            dtype=mdtype)
     fused = isinstance(net, d.FusedDistributedFNO)
     d.print0(f"backend = {'fused sm_90a engine' if fused else 'portable (torch.fft / torch.distributed)'}, dtype = {mdtype}")
-    params = [p for p in net.parameters() if p.numel() > 0]
     criterion, mse = d.DistributedMSELoss(P_x).to(device), d.DistributedMSELoss(P_x).to(device)
-    optimizer = (d.FusedAdam(net, lr=1e-3, weight_decay=1e-4) if fused
-                 else torch.optim.Adam(params, lr=1e-3, weight_decay=1e-4))
+    optimizer, scheduler, clip = d.make_optimizer(net, args, fused, lr=1e-3, weight_decay=1e-4, group=P_x.group)
     if not fused:                                   # the fused engine takes fp32 / bf16 inputs as they are
         x_train, x_test = x_train.to(mdtype), x_test.to(mdtype)
     steps, train_accs, test_accs = [], [], []
@@ -119,9 +118,13 @@ with ctx:
             y = d.unit_gaussian_denormalize(y_train[a:b], mu_y, std_y)
             loss = criterion(y_hat, y)
             loss.backward()
+            if clip is not None:
+                clip()
             optimizer.step()
             if P_0.active:
                 tl, nb = tl + loss.item(), nb + 1
+        if scheduler is not None:
+            scheduler.step()
         if P_0.active:
             print(f"epoch = {i}, average train loss = {tl / max(nb, 1)}")
             steps.append(i); train_accs.append(tl / max(nb, 1))
@@ -139,7 +142,7 @@ with ctx:
             print(f"average test loss = {te / max(nt_, 1)}\naverage test mse  = {tm / max(nt_, 1)}")
             test_accs.append(te / max(nt_, 1))
         if (i + 1) % args.checkpoint_interval == 0:
-            path = d.save_checkpoint(net, str(out_dir), epoch=i + 1, optimizer=optimizer)
+            path = d.save_checkpoint(net, str(out_dir), epoch=i + 1, optimizer=optimizer, scheduler=scheduler)
             print(f"saved model: {Path(path).resolve()}")
             if y_true:
                 np.savez(out_dir / f"mat_{i + 1:04d}_{max(P_x.rank, 0):04d}.npz",

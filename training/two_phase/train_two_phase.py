@@ -36,6 +36,7 @@ ap.add_argument("--data-dir", default=None, help="directory of <name>_<i>.npy fi
 ap.add_argument("--cache-dir", default=None)
 ap.add_argument("--resume", action="store_true")
 ap.add_argument("--dtype", default="auto", choices=["auto", "bf16", "fp32"])
+d.add_optimizer_args(ap)
 args = ap.parse_args()
 
 d.ensure_process_group()
@@ -60,16 +61,15 @@ with ctx:
     fused = isinstance(net, d.FusedDistributedFNO)
     d.print0(f"backend = {'fused sm_90a engine' if fused else 'portable (torch.fft / torch.distributed)'}, dtype = {dtype}")
     criterion = d.DistributedRelativeLpLoss(P_x).to(device)
-    params = [p for p in net.parameters() if p.numel() > 0]
-    optimizer = d.FusedAdam(net, lr=args.lr) if fused else (torch.optim.Adam(params, lr=args.lr) if params else None)
-    trainer = d.Trainer(net, criterion, optimizer, device=device) if optimizer is not None else None
+    optimizer, scheduler, clip = d.make_optimizer(net, args, fused, lr=args.lr, group=P_x.group)
+    trainer = d.Trainer(net, criterion, optimizer, device=device, before_step=clip) if optimizer is not None else None
     start, hist = 0, {"train": [], "valid": []}
     log = d.get_logger("two_phase")
     metrics = d.MetricsWriter(args.out_dir)                 # metrics_0000.jsonl on the root
     if args.resume:
         last = d.latest_checkpoint(args.out_dir, max(P_x.rank, 0))
         if last is not None:
-            info = d.load_checkpoint(net, args.out_dir, epoch=last, optimizer=optimizer)
+            info = d.load_checkpoint(net, args.out_dir, epoch=last, optimizer=optimizer, scheduler=scheduler)
             start, hist = last, info.get("history", hist)
             if P_root.active:
                 print(f"resumed from epoch {last}")
@@ -88,6 +88,8 @@ with ctx:
             if j % 50 == 0:
                 log.info(f"epoch = {epoch}, batch = {j}, loss = {loss:.6f}, dt = {time.time() - t0:.3f}")
                 metrics.log(step=epoch * len(train_loader) + j, epoch=epoch, loss=loss, dt=time.time() - t0)
+        if scheduler is not None:
+            scheduler.step()
         net.eval()
         vtot, vbat = 0.0, 0
         for x, y in valid_loader:
@@ -97,13 +99,14 @@ with ctx:
             log.info(f"epoch = {epoch}, train loss = {hist['train'][-1]:08f}, val loss = {hist['valid'][-1]:08f}")
             metrics.log(epoch=epoch, train_loss=hist["train"][-1], valid_loss=hist["valid"][-1])
         if (epoch + 1) % args.checkpoint_interval == 0:
-            path = d.save_checkpoint(net, args.out_dir, epoch=epoch + 1, optimizer=optimizer,
+            path = d.save_checkpoint(net, args.out_dir, epoch=epoch + 1, optimizer=optimizer, scheduler=scheduler,
                                      extra={"history": hist, "plan": "fused" if fused else "reference"})
             if P_root.active:
                 with open(os.path.join(args.out_dir, f"loss_epoch_{epoch}.json"), "w") as f:
                     json.dump(hist, f)
             print(f"rank = {P_x.rank}, saved model: {path}")
-    path = d.save_checkpoint(net, args.out_dir, epoch=None, optimizer=optimizer, extra={"history": hist})
+    path = d.save_checkpoint(net, args.out_dir, epoch=None, optimizer=optimizer, scheduler=scheduler,
+                             extra={"history": hist})
     print(f"rank = {P_x.rank}, saved model after final iteration: {path}")
     metrics.close()
     d.print0("training finished.")
