@@ -40,6 +40,7 @@ import torch.nn as nn
 
 from ..ops import operators as OPS
 from ..ops.gemm import DFT_GEMM_SMEM, ScatterSpec, dft_gemm_fits, dft_gemm_min_smem, pad_operator
+from ..parallel.decomposition import balanced_bounds
 from ..parallel.partition import Partition
 
 __all__ = ["FusedDistributedFNO", "FusedAdam", "supports", "wants", "EnginePlan", "fold_onto_pencil",
@@ -87,10 +88,51 @@ def _pencil_axis(grid: Sequence[int]) -> Optional[int]:
     return None
 
 
+def pencil_storage(Y: int, KZ: int, P: int) -> Tuple[int, int]:
+    """Per-rank storage ``(Yl, kzl)`` of the y rows and the kz modes on a P-rank y-pencil.  Where P divides an axis
+    this is the share.  Otherwise every rank still stores one uniform extent, so that the kernels, scatter specs and
+    peer layouts keep uniform strides, and the entries past a rank's share of the balanced decomposition are dead:
+    the smallest extent >= the largest share that the kernels take -- y rows in multiples of 4 (spectral_in clips its
+    stores in 16-byte units), kz modes such that ``P * kzl`` is a multiple of 4 (the inverse z-DFT reads rows of
+    ``2 * KZ`` bf16, a whole number of 16-byte units)."""
+    Yl = Y // P if Y % P == 0 else (-(-Y // P) + 3) // 4 * 4
+    if KZ % P == 0:
+        return Yl, KZ // P
+    kzl = -(-KZ // P)
+    while P * kzl % 4:
+        kzl += 1
+    return Yl, kzl
+
+
+def _storage_map(n: int, P: int, per: int) -> List[int]:
+    """Storage index -> global index of an axis of ``n`` entries over ``P`` ranks that store ``per`` entries each:
+    rank r's live entries are its balanced share, in order; the rest are dead (-1)."""
+    out: List[int] = []
+    for r in range(P):
+        a, b = balanced_bounds(n, P, r)
+        out += list(range(a, b)) + [-1] * (per - (b - a))
+    return out
+
+
+def _pairs_to_storage(op: torch.Tensor, index: Sequence[int], axis: int) -> torch.Tensor:
+    """``op`` with its interleaved (re, im) axis ``axis`` re-indexed to storage: pair s is pair ``index[s]`` of ``op``,
+    or zeros where ``index[s] < 0`` (a dead entry)."""
+    if axis == 1:
+        return _pairs_to_storage(op.t(), index, 0).t().contiguous()
+    idx = torch.tensor(index, dtype=torch.long)
+    live = idx >= 0
+    src = op.reshape(op.shape[0] // 2, 2, op.shape[1])
+    out = torch.zeros(len(index), 2, op.shape[1], dtype=op.dtype)
+    out[live] = src[idx[live]]
+    return out.reshape(2 * len(index), op.shape[1])
+
+
 def fold_onto_pencil(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, out_channels: int = 1):
     """``(P_work, R_in, R_out)``: the y-pencil over ``P_x``'s ranks and the two re-shards that move
     the network input onto it and the ``out_channels``-channel output back (``None`` when ``P_x`` already is that
-    pencil).  Both re-shards move the unpadded tensors: a network with ``padding`` pads after its lift, on the pencil."""
+    pencil).  Both re-shards move the unpadded tensors: a network with ``padding`` pads after its lift, on the pencil.
+    The pencil may be ragged (e.g. ``(1,1,2,3,1,1)`` folded onto 6 GPUs): both re-shards target its balanced
+    decomposition, which is exactly the engine's live rows (:class:`EnginePlan`), so no further re-shard is needed."""
     if _pencil_axis(P_x.shape) is not None:
         return P_x, None, None
     from ..parallel.primitives import Repartition
@@ -117,7 +159,11 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
 
     ``padding`` (see :class:`dfno_b200.models.fno.DistributedFNO`) runs on the round-2 route only; the engine's y axis
     (the pencil axis) can be padded at one rank only, z in multiples of 8, t by an even count.  Every other limit
-    applies to the padded extents.  Malformed ``padding`` raises ``ValueError``."""
+    applies to the padded extents.  Malformed ``padding`` raises ``ValueError``.
+
+    A y extent or a kz mode count ``2 * modes_z`` that P does not divide runs on uniform per-rank storage whose
+    entries past each rank's balanced share are dead (:func:`pencil_storage`).  Dead y rows need the padded lift and
+    head, so a ragged y axis runs on the round-2 route only; the extent limits apply to the stored rows."""
     from .fno import check_out_channels, check_padding
     O = check_out_channels(out_channels)
     six = _as_6d(P_x.shape, in_shape, modes)
@@ -132,9 +178,13 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
     B, Cin, X, Y, Z, Tin = shape6
     T = int(out_timesteps)
     mx, my, mz, mt = modes6
+    # a grid or mode count that P does not divide runs on uniform per-rank storage with dead entries (pencil_storage);
+    # the route checks below take the stored kz count, which the kernels see
+    KZs = P * pencil_storage(Y, 2 * mz, P)[1]
+    kz_here = f"here {2 * KZs}" + (f": {2 * mz} kz modes stored as {KZs} on {P} GPUs" if KZs != 2 * mz else "")
     if pad is not None:
-        if 2 * (2 * mz) > 128:
-            return False, (f"padding {list(pad)} needs the round-2 route (2 * 2 * modes_z <= 128, here {4 * mz}); the "
+        if 2 * KZs > 128:
+            return False, (f"padding {list(pad)} needs the round-2 route (2 * 2 * modes_z <= 128, {kz_here}); the "
                            f"round-1 head has no padded layout")
         if pad6[1] and P > 1:
             return False, (f"padding {list(pad)} pads the axis the engine splits over {P} GPUs "
@@ -149,19 +199,20 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
         return False, f"width {width} not in {SUPPORTED_WIDTHS} (nor in {WIDE_WIDTHS}, the round-2 widths)"
     if O > MAX_OUT:
         return False, f"out_channels = {O}: the fused projection head covers 1 <= out_channels <= {MAX_OUT}"
-    if O > 1 and 2 * (2 * mz) > 128:
-        return False, (f"out_channels = {O} needs the round-2 route (2 * 2 * modes_z <= 128, here {4 * mz}); the "
+    if O > 1 and 2 * KZs > 128:
+        return False, (f"out_channels = {O} needs the round-2 route (2 * 2 * modes_z <= 128, {kz_here}); the "
                        f"round-1 head is single-output")
     if O > 1 and width > 31:
         return False, (f"out_channels = {O} at width {width}: the multi-output head backward covers width <= 31 "
                        f"(its consumer registers run out at 32)")
-    if width in WIDE_WIDTHS and 2 * (2 * mz) > 128:
-        return False, (f"width {width} needs the round-2 route (2 * 2 * modes_z <= 128, here {4 * mz}); the round-1 "
+    if width in WIDE_WIDTHS and 2 * KZs > 128:
+        return False, (f"width {width} needs the round-2 route (2 * 2 * modes_z <= 128, {kz_here}); the round-1 "
                        f"kernels cover widths {SUPPORTED_WIDTHS}")
     if P > 8:
         return False, "at most 8 peers (one NVSwitch box)"
-    if Y % P or (2 * mz) % P:
-        return False, "Y and 2*modes_z must divide evenly over the pencil"
+    if Y % P and 2 * KZs > 128:
+        return False, (f"{'X' if five_d else 'Y'} = {Y} over {P} GPUs leaves dead rows, which need the round-2 route "
+                       f"(2 * 2 * modes_z <= 128, {kz_here}); the round-1 head has no padded layout")
     if Cin > MAX_IN or Tin > 64:
         return False, f"lift kernels cover Cin <= {MAX_IN} and Tin <= 64"
     lift_w = (T - pad6[3]) * Tin + (T - pad6[3]) + 2 * (width * Cin + width)    # linear1 maps Tin -> the interior T
@@ -170,14 +221,16 @@ def supports(P_x: Partition, in_shape: Sequence[int], out_timesteps: int, width:
                        f"{LIFT_MAX_W} (kLiftMaxW)")
     # T % 4 != 0 (e.g. the reference's two-phase run and in-module demo, T = 30) uses a padded t pitch in Z1
     # (EnginePlan.Tp); covered by tests/test_fused_gpu.py.  T = 1 runs the chain without t stages (EnginePlan.has_t).
-    if Z % 8 or (T % 2 and T != 1) or Y % 4 or (X % 4 and X != 1) or (mx % 2 and X != 1) or my % 2 or mz % 2:
+    Ys = P * pencil_storage(Y, 2 * mz, P)[0]     # the stored y rows the y stages transform (Y when P divides it)
+    if Z % 8 or (T % 2 and T != 1) or Ys % 4 or (X % 4 and X != 1) or (mx % 2 and X != 1) or my % 2 or mz % 2:
         return False, ("extents must satisfy Z%8 = T%2 = X%4 = Y%4 = 0 (T = 1 or even) and even modes "
                        "(TMA pitch alignment)")
     if (X != 1 and 2 * mx > X) or 2 * my > Y or 2 * mz > Z or mt > T // 2 + 1:
         return False, "mode counts exceed the axes"
-    if max(Z, 2 * T) > 256 or max(2 * X, 2 * Y) > 512:
-        return False, "transformed axes: Z <= 256, T <= 128, X, Y <= 256 samples"
-    if B * width * X * (Y // P) * Z * T >= 2 ** 31:
+    if max(Z, 2 * T) > 256 or max(2 * X, 2 * Ys) > 512:
+        return False, ("transformed axes: Z <= 256, T <= 128, X, Y <= 256 samples"
+                       + (f" (Y over {P} GPUs is stored as {Ys} rows)" if Ys != Y else ""))
+    if B * width * X * (Ys // P) * Z * T >= 2 ** 31:
         return False, "per-rank activation must stay below 2^31 elements"
     pl = EnginePlan(B, Cin, Tin, width, T - pad6[3], X - pad6[0], Y - pad6[1], Z - pad6[2], modes6, world=P, rank=0,
                     out_channels=O, pad=pad6)
@@ -242,25 +295,33 @@ class EnginePlan:
         # pad (px, py, pz, pt): zeros appended to the lifted field.  X, Y, Z, T below are the padded extents everything
         # between the lift and the head runs on; the network input and output keep the interior ones Xi, Yi, Zi, Ti.
         self.pad = tuple(int(p) for p in pad) if pad else (0, 0, 0, 0)
-        self.padded = any(self.pad)
         self.Xi, self.Yi, self.Zi, self.Ti = X, Y, Z, T
-        self.Yli = Y // world
+        # live y rows of this rank: its share of the balanced decomposition (that of the network's input shard)
+        self.y_off, y_end = balanced_bounds(Y, world, rank)
+        self.Yli = y_end - self.y_off
         X, Y, Z, T = X + self.pad[0], Y + self.pad[1], Z + self.pad[2], T + self.pad[3]
         self.B, self.Cin, self.Tin, self.C, self.T = B, Cin, Tin, C, T
         self.O = int(out_channels)                         # output channels (fields) of the head
-        self.X, self.Y, self.Z = X, Y, Z
         self.mx, self.my, self.mz, self.mt = [int(m) for m in modes]
         self.world, self.rank, self.H = world, rank, hidden
         self.max_n = MAX_N                                 # widest operator one GEMM launch keeps resident
-        self.Yl = Y // world
-        self.y_off = rank * self.Yl
         self.has_x = X > 1                                 # X == 1: 2-D + time problem, no x transform (see _as_6d)
         # T == 1 (steady problem / next-step prediction): the t-DFT and its inverse are identities on the single bin,
         # so the chain has no G1b / iG1b, G1a scatters straight into S1 and iG2's T1 already is the last stage's input
         self.has_t = T > 1
-        self.KX, self.KY, self.KZ = (2 * self.mx if self.has_x else 1), 2 * self.my, 2 * self.mz
-        self.kzl = self.KZ // world
-        self.kz_off = rank * self.kzl
+        self.KX, self.KY = (2 * self.mx if self.has_x else 1), 2 * self.my
+        # Storage vs live (pencil_storage).  Every rank stores Yl y rows and kzl kz modes; Y and KZ are the stored
+        # totals the chain runs on, Yg and KZg the true ones.  Live kz of this rank: its balanced share of the KZg
+        # modes.  The operators (operators()) carry zeros at the dead entries, so a dead y row of an activation and a
+        # dead kz mode of a spectrum stay exactly zero.  When P divides both axes, storage is live and nothing is dead.
+        self.Yg, self.KZg = Y, 2 * self.mz
+        self.Yl, self.kzl = pencil_storage(Y, self.KZg, world)
+        self.Y, self.KZ = world * self.Yl, world * self.kzl
+        self.kz_off, kz_end = balanced_bounds(self.KZg, world, rank)
+        self.kzl_live = kz_end - self.kz_off
+        self.X, self.Z = X, Z
+        # rows past the interior (padding, or dead rows): the lift writes them as zeros and the head skips them
+        self.padded = any(self.pad) or self.Yli != self.Yl
         self.mtp = (self.mt + 3) // 4 * 4 if self.has_t else 1    # kt pitch of T1 (iG1b reads 16-byte rows)
         self.Tp = (T + 3) // 4 * 4                         # t pitch of Z1: G1b reads rows of 2*Tp bf16 (16-byte TMA pitch)
         self.BC = B * C
@@ -282,7 +343,7 @@ class EnginePlan:
         self.n_act = BC * self.S
         # Z1 (G1a -> G1b) and U (iG1b -> last stage) exist only for the t stages: at T == 1 T1 is U's layout
         self.n_Z1 = BC * X * self.KZ * Yl * self.Tp * 2 if self.has_t else 0
-        self.n_S1 = BC * kzl * mt * X * Y * 2
+        self.n_S1 = BC * kzl * mt * X * self.Y * 2
         self.n_S2 = BC * kzl * mt * self.KY * X * 2
         self.n_S3 = BC * self.Q * 2
         self.n_T2 = BC * X * kzl * mt * self.KY * 2
@@ -321,6 +382,14 @@ class EnginePlan:
         self.n_theta = off
         self.num_blocks = num_blocks
 
+    def theta_meta(self, ndim: int = 6) -> Dict[str, object]:
+        """What interprets this rank's flat ``theta`` (see ``FusedDistributedFNO.engine_meta``): the segment table
+        and the spectral shard's stored (``kzl``) and live (``kzl_live`` from ``kz_off``) kz modes."""
+        return {"format": "fused-theta", "segments": dict(self.segments), "C": self.C, "kzl": self.kzl,
+                "kz_off": self.kz_off, "kzl_live": self.kzl_live, "mt": self.mt, "KX": self.KX, "KY": self.KY,
+                "KZ": self.KZg, "rank": self.rank, "world": self.world, "num_blocks": self.num_blocks, "ndim": ndim,
+                "out_channels": self.O}
+
     # ---------------------------------------------------------------- stage descriptors
     def chain(self, staged: bool = False) -> List[dict]:
         """The GEMM stages of one spectral convolution (forward *or* adjoint: only the operator
@@ -344,7 +413,7 @@ class EnginePlan:
                 st.append(dict(name="G1a", src="src", dst="S1", M=BC * X * Yl, K=Z, lda=Z, N=2 * KZ, op="G1a",
                                scatter=ScatterSpec(rows=[(Yl, 2), (X, Y * 2), (BC, kzl * X * Y * 2)],
                                                    cols=(kzl, X * Y * 2, 0), peer=("col", kzl),
-                                                   base_off=self.y_off * 2),
+                                                   base_off=r * Yl * 2),
                                peer_dst=True, barrier_after=True))
             else:               # S1s[bc, kz', r_src, x, y_loc, ri]
                 st.append(dict(name="G1a", src="src", dst="S1s", M=BC * X * Yl, K=Z, lda=Z, N=2 * KZ, op="G1a",
@@ -358,7 +427,7 @@ class EnginePlan:
                                                cols=(KZ, Yl * Tp * 2, 0))))
             st.append(dict(name="G1b", src="Z1", dst="S1", M=BC * X * KZ * Yl, K=2 * T, lda=2 * Tp, N=2 * mt, op="G1b",
                            scatter=ScatterSpec(rows=[(Yl, 2), (KZ, mt * X * Y * 2), (X, Y * 2), (BC, m_loc * X * Y * 2)],
-                                               cols=(mt, X * Y * 2, 0), peer=("row", 1, kzl), base_off=self.y_off * 2),
+                                               cols=(mt, X * Y * 2, 0), peer=("row", 1, kzl), base_off=r * Yl * 2),
                            peer_dst=True, barrier_after=True))
         else:
             st.append(dict(name="G1a", src="src", dst="Z1", M=BC * X * Yl * T, K=Z, lda=Z, N=2 * KZ, op="G1a",
@@ -392,7 +461,7 @@ class EnginePlan:
                            scatter=ScatterSpec(rows=[(mt, 2), (kzl, mtp * 2), (X, Yl * KZ * mtp * 2),
                                                      (BC, X * Yl * KZ * mtp * 2)],
                                                cols=(Yl, KZ * mtp * 2, 0), peer=("col", Yl),
-                                               base_off=self.kz_off * mtp * 2),
+                                               base_off=r * kzl * mtp * 2),
                            peer_dst=True, barrier_after=True))
         else:
             st.append(dict(name="iG2", src="T2" if self.has_x else "S4", dst="T1s", M=BC * X * m_loc, K=2 * KY,
@@ -526,14 +595,30 @@ class EnginePlan:
                 "hbm_floor_ms": hbm / (hbm_gbs * 1e9) * 1e3,
                 "nvlink_ms": (link / (nvlink_gbs * 1e9) * 1e3 if link else 0.0) if nvlink_gbs else None}
 
+    def y_map(self) -> List[int]:
+        """Stored y row (all ranks, rank-major) -> true global y, -1 for a dead row."""
+        return _storage_map(self.Yg, self.world, self.Yl)
+
+    def kz_map(self) -> List[int]:
+        """Stored kz mode (all ranks, rank-major) -> index among the ``KZg`` retained kz modes, -1 for a dead mode."""
+        return _storage_map(self.KZg, self.world, self.kzl)
+
     def operators(self) -> Dict[str, torch.Tensor]:
-        """Forward-chain operators (float64) and their adjoint-chain counterparts (``*_adj``)."""
-        X, Y, Z, T = self.X, self.Y, self.Z, self.T
+        """Forward-chain operators (float64) and their adjoint-chain counterparts (``*_adj``).  On ragged storage
+        the y-DFT reads no dead row and its inverse writes zeros there, the z-DFT writes zeros at dead kz and its
+        inverse reads none; the basis is the true length-``Yg`` / length-``Z`` DFT at each live entry's global index."""
+        X, Y, Z, T = self.X, self.Yg, self.Z, self.T
         f = {
             "G1a": OPS.fwd_real_to_complex(Z, self.mz), "G1b": OPS.fwd_complex(T, self.mt, False),
             "G2": OPS.fwd_complex(Y, self.my), "iG2": OPS.inv_complex(Y, self.my),
             "iG1b": OPS.inv_complex_hermitian(T, self.mt), "iG1a": OPS.inv_complex_to_real(Z, self.mz),
         }
+        if self.Y != self.Yg:
+            ym = self.y_map()
+            f["G2"], f["iG2"] = _pairs_to_storage(f["G2"], ym, 1), _pairs_to_storage(f["iG2"], ym, 0)
+        if self.KZ != self.KZg:
+            km = self.kz_map()
+            f["G1a"], f["iG1a"] = _pairs_to_storage(f["G1a"], km, 0), _pairs_to_storage(f["iG1a"], km, 1)
         mirror = {"G1a": "iG1a", "G1b": "iG1b", "G2": "iG2", "iG2": "G2", "iG1b": "G1b", "iG1a": "G1a"}
         if not self.has_t:       # at T == 1 both t operators are the 2 x 2 identity: the chain has no t stages
             for k in ("G1b", "iG1b"):
@@ -766,7 +851,7 @@ class FusedDistributedFNO(nn.Module):
             off = r * X * Yl * 2
         else:                # S1[bc, kz', kt, x, y, ri]
             dstr = [Y * 2, X * Y * 2, mt * X * Y * 2, kzl * mt * X * Y * 2]
-            off = pl.y_off * 2
+            off = r * Yl * 2
         if "G1a" not in self.ops or "G1b" not in self.ops:
             return None
         o1, o2 = self.ops["G1a"], self.ops["G1b"]
@@ -807,16 +892,17 @@ class FusedDistributedFNO(nn.Module):
             for name, (off, shape) in pl.segments.items():
                 t = self._seg(name)
                 if name.endswith(".spectral"):
+                    slab = t.view(pl.C, pl.C, pl.kzl, pl.mt * pl.KY * pl.KX, 2)
                     if seed is None:
                         t.copy_(torch.rand(shape, device=self.device) / (self.width * self.width))
                     else:
                         k = int(name.split(".")[1])
-                        slab = t.view(pl.C, pl.C, pl.kzl, pl.mt * pl.KY * pl.KX, 2)
                         g2 = torch.Generator(device=self.device)
-                        for j in range(pl.kzl):
+                        for j in range(pl.kzl_live):
                             g2.manual_seed(int(seed) * 1000003 + k * 4099 + pl.kz_off + j + 1)
                             slab[:, :, j] = torch.rand(pl.C, pl.C, slab.shape[3], 2, device=self.device,
                                                        generator=g2) / (self.width * self.width)
+                    slab[:, :, pl.kzl_live:] = 0                # dead kz modes (ragged storage) hold no weight
                 elif name.endswith(".W"):
                     if seed is None:
                         nn.init.kaiming_uniform_(t, a=math.sqrt(5))
@@ -1192,24 +1278,23 @@ class FusedDistributedFNO(nn.Module):
     def engine_meta(self) -> Dict[str, object]:
         """What is needed to interpret this rank's flat ``theta`` outside the module (stored next to per-rank
         checkpoints so that fused checkpoints can be assembled / re-sharded offline)."""
-        pl = self.plan
-        return {"format": "fused-theta", "segments": dict(pl.segments), "C": pl.C, "kzl": pl.kzl, "kz_off": pl.kz_off,
-                "mt": pl.mt, "KX": pl.KX, "KY": pl.KY, "KZ": pl.KZ, "rank": self.rank, "world": self.world,
-                "num_blocks": self.num_blocks, "ndim": len(self.in_shape), "out_channels": pl.O,
+        return {**self.plan.theta_meta(len(self.in_shape)),
                 "padding": None if self.padding is None else list(self.padding)}
 
     @staticmethod
     def theta_to_canonical(theta: torch.Tensor, meta: Dict[str, object], include_pointwise: bool = True):
         """This rank's part of the canonical state from a flat ``theta`` (CPU tensor) and its :meth:`engine_meta`:
         ``{name: tensor}`` for pointwise weights, ``{name: (kz_off, slab)}`` for spectral shards (global layout
-        ``[i, o, KX, KY, kzl, mt]``)."""
+        ``[i, o, KX, KY, kzl_live, mt]``: the live kz modes only).  Also maps a tensor laid out like ``theta``, such as
+        :class:`FusedAdam`'s moments."""
         out = {}
         C, kzl, mt, KX, KY = (int(meta[k]) for k in ("C", "kzl", "mt", "KX", "KY"))
+        live = int(meta.get("kzl_live", kzl))
         for name, (off, shape) in meta["segments"].items():
             t = theta[off:off + int(np.prod(shape))].view(shape).detach().cpu()
             if name.endswith(".spectral"):
-                # native [i, o, kzl, mt, KY, KX, 2] -> global slab [i, o, KX, KY, kzl, mt]
-                w = torch.view_as_complex(t.reshape(C, C, kzl, mt, KY, KX, 2).contiguous())
+                # native [i, o, kzl, mt, KY, KX, 2] -> global slab [i, o, KX, KY, kzl_live, mt]
+                w = torch.view_as_complex(t.reshape(C, C, kzl, mt, KY, KX, 2)[:, :, :live].contiguous())
                 out[name] = (int(meta["kz_off"]), w.permute(0, 1, 5, 4, 2, 3).contiguous())
             elif include_pointwise:
                 tt = t
@@ -1259,27 +1344,39 @@ class FusedDistributedFNO(nn.Module):
         """Load a canonical state.  ``strict``: every engine segment must be present; otherwise missing segments
         keep their values -- but a state that matches NO segment is always an error (it used to load nothing,
         silently)."""
-        pl = self.plan
-        missing = [n for n in pl.segments if n not in state]
-        if missing and (strict or len(missing) == len(pl.segments)):
-            raise KeyError(f"canonical state lacks {len(missing)} of {len(pl.segments)} engine segments, e.g. "
+        self.canonical_to_theta(state, self.engine_meta(), self.theta.data, strict=strict)
+
+    @staticmethod
+    def canonical_to_theta(state, meta: Dict[str, object], theta: torch.Tensor, strict: bool = True) -> None:
+        """Write this rank's part of a canonical state into a flat ``theta`` (or a tensor laid out like it, such as
+        :class:`FusedAdam`'s moments), described by its :meth:`engine_meta`; the inverse of :meth:`theta_to_canonical`.
+        Dead kz modes (ragged storage) are set to zero.  ``strict`` as in :meth:`engine_state_from_global`."""
+        segments = meta["segments"]
+        missing = [n for n in segments if n not in state]
+        if missing and (strict or len(missing) == len(segments)):
+            raise KeyError(f"canonical state lacks {len(missing)} of {len(segments)} engine segments, e.g. "
                            f"{missing[:3]} (keys present: {sorted(state)[:4]}...)")
+        kzl, kz_off = int(meta["kzl"]), int(meta["kz_off"])
+        live = int(meta.get("kzl_live", kzl))
         with torch.no_grad():
-            for name, (off, shape) in pl.segments.items():
+            for name, (off, shape) in segments.items():
                 if name not in state:
                     continue
                 src = state[name]
+                dst = theta[off:off + int(np.prod(shape))]
                 if name.endswith(".spectral"):
-                    if self.five_d and src.dim() == 5:
+                    if int(meta.get("ndim", 6)) == 5 and src.dim() == 5:
                         src = src.unsqueeze(2)
-                    w = src[:, :, :, :, pl.kz_off:pl.kz_off + pl.kzl, :].to(torch.complex64)
-                    w = torch.view_as_real(w.permute(0, 1, 4, 5, 3, 2).contiguous())   # [i,o,kzl,mt,KY,KX,2]
-                    self._seg(name).copy_(w.reshape(shape).to(self.device))
+                    w = src[:, :, :, :, kz_off:kz_off + live, :].to(torch.complex64)
+                    w = torch.view_as_real(w.permute(0, 1, 4, 5, 3, 2).contiguous())   # [i,o,kzl_live,mt,KY,KX,2]
+                    if live < kzl:
+                        w = torch.cat([w, w.new_zeros(w.shape[0], w.shape[1], kzl - live, *w.shape[3:])], dim=2)
+                    dst.copy_(w.reshape(-1).to(dst.device))
                 else:
                     if src.numel() != int(np.prod(shape)):
                         raise ValueError(f"canonical state entry {name} has shape {list(src.shape)}, this engine needs "
-                                         f"{list(shape)} (out_channels = {pl.O})")
-                    self._seg(name).copy_(src.reshape(shape).to(self.device, torch.float32))
+                                         f"{list(shape)} (out_channels = {meta.get('out_channels', 1)})")
+                    dst.copy_(src.reshape(-1).to(dst.device, torch.float32))
 
 
 # =====================================================================================

@@ -51,13 +51,15 @@ def main():
     for g in grid:
         P *= g
     pad = a.padding or (0, 0, 0, 0)
-    if (Y + pad[1]) % P or (2 * a.modes[2]) % P:
-        return 0 if ok else 1
     pl = EnginePlan(a.batch, a.in_channels, a.in_timesteps, a.width, T, X, Y, Z, a.modes, world=P, rank=0,
                     out_channels=a.out_channels, pad=pad)
     pl.finish(a.blocks)
     if tuple(grid) != (1, 1, 1, P, 1, 1):
         print(f"work partition: (1, 1, 1, {P}, 1, 1) (input / output re-sharded once per step)")
+    # ragged pencil: every rank stores the same extents, the entries past its balanced share are dead work
+    print(f"y rows: {pl.Yl} stored per rank, {pl.Y} in all for {pl.Yg} live (storage / live {pl.Y / pl.Yg:.4f}, "
+          f"dead fraction {1 - pl.Yg / pl.Y:.2%});  kz modes: {pl.kzl} stored per rank, {pl.KZ} in all for {pl.KZg} "
+          f"live (storage / live {pl.KZ / pl.KZg:.4f}, dead fraction {1 - pl.KZg / pl.KZ:.2%})")
     for train in (True, False):
         m = pl.memory_bytes(train=train)
         print(f"\nper-rank memory, {'training' if train else 'inference'} "
