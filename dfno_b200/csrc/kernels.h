@@ -120,6 +120,13 @@ const char* scaled_diff(const float* yh, const float* y, const float* scale, flo
 const char* spectral_out(const void* U, const void* h, const void* Bop, int n_pad, int k_pad, const float* W,
                          int transpose_w, void* pre, void* out, int B, int C, long long L, int Z, int K1, int gelu,
                          int save_pre, int num_sms, cudaStream_t stream);
+// The adjoint of spectral_out with the pointwise backward of the neighbouring blocks folded in: pre_prev (may be null)
+// is pre_{k-1} in and dpre_{k-1} = g * gelu'(pre_{k-1}) out (g is then not stored), h + dW (may be null): dW += dpre . h^T.
+// spectral_out_adj_check: null when the kernel takes the shape (dpre / dw: which of the two it folds), the reason otherwise.
+const char* spectral_out_adj(const void* U, const void* dpre, const void* Bop, int n_pad, int k_pad, const float* W,
+                             void* pre_prev, void* g, const void* h, float* dW, int B, int C, long long L, int Z, int K1,
+                             int num_sms, cudaStream_t stream);
+const char* spectral_out_adj_check(int n_pad, int k_pad, int C, int Z, int K1, int dpre, int dw);
 // dpre = g * gelu'(pre) (in place over pre); dW += dpre . h^T
 const char* dpre_dw(const void* g, void* pre_dpre, const void* h, float* dW, int B, int C, long long L, int Z,
                     int num_sms, cudaStream_t stream);

@@ -270,15 +270,35 @@ void fft_radix(const at::Tensor& x, at::Tensor& y, int64_t N, int64_t lines, boo
                         inverse, in_real, out_real, one_sided, static_cast<int>(m), sm_count(), cur_stream()), "fft_radix");
 }
 
+// pre_prev / h_dw / dW (adjoint only, optional): fold the neighbouring pointwise backward into the adjoint
+// (spectral_out_adj); with pre_prev, `out` is not written
 void spectral_out(const at::Tensor& U, const at::Tensor& h, const at::Tensor& Bop, const at::Tensor& W, bool transpose_w,
                   const c10::optional<at::Tensor>& pre, at::Tensor& out, int64_t B, int64_t C, int64_t L, int64_t Z,
-                  int64_t K1, bool gelu, bool save_pre) {
+                  int64_t K1, bool gelu, bool save_pre, const c10::optional<at::Tensor>& pre_prev,
+                  const c10::optional<at::Tensor>& h_dw, const c10::optional<at::Tensor>& dW) {
   TORCH_CHECK(Bop.dim() == 2 && Bop.is_contiguous(), "operator must be a contiguous [n_pad, k_pad] tensor");
   c10::cuda::CUDAGuard guard(U.device());
+  if (pre_prev || h_dw || dW) {
+    TORCH_CHECK(transpose_w && !gelu, "pre_prev / h_dw / dW: adjoint only");
+    TORCH_CHECK(!dW || (dW->scalar_type() == at::kFloat && dW->numel() >= C * C), "dW: fp32 [C, C]");
+    check(dfno::spectral_out_adj(bptr(U), bptr(h), bptr(Bop), static_cast<int>(Bop.size(0)),
+                                 static_cast<int>(Bop.size(1)), fptr(W), pre_prev ? bptr(*pre_prev) : nullptr, bptr(out),
+                                 h_dw ? bptr(*h_dw) : nullptr, dW ? const_cast<float*>(fptr(*dW)) : nullptr, static_cast<int>(B),
+                                 static_cast<int>(C), L, static_cast<int>(Z), static_cast<int>(K1), sm_count(),
+                                 cur_stream()), "spectral_out_adj");
+    return;
+  }
   check(dfno::spectral_out(bptr(U), bptr(h), bptr(Bop), static_cast<int>(Bop.size(0)), static_cast<int>(Bop.size(1)),
                            fptr(W), transpose_w ? 1 : 0, pre ? bptr(*pre) : nullptr, bptr(out), static_cast<int>(B),
                            static_cast<int>(C), L, static_cast<int>(Z), static_cast<int>(K1), gelu ? 1 : 0,
                            save_pre ? 1 : 0, sm_count(), cur_stream()), "spectral_out");
+}
+
+// "" when the folded adjoint takes the shape, the reason otherwise (no launch, no device needed)
+std::string spectral_out_adj_check(int64_t n_pad, int64_t k_pad, int64_t C, int64_t Z, int64_t K1, bool dpre, bool dw) {
+  const char* e = dfno::spectral_out_adj_check(static_cast<int>(n_pad), static_cast<int>(k_pad), static_cast<int>(C),
+                                               static_cast<int>(Z), static_cast<int>(K1), dpre ? 1 : 0, dw ? 1 : 0);
+  return e ? std::string(e) : std::string();
 }
 
 void spectral_in(const at::Tensor& h, const at::Tensor& op1, const at::Tensor& op2, const std::vector<int64_t>& dst_ptrs,
@@ -445,7 +465,11 @@ void register_ops(pybind11::module& m) {
   m.def("spectral_in", &spectral_in);
   m.def("spectral_in_check", &spectral_in_check);
   m.def("spectral_in_config", &spectral_in_config);
-  m.def("spectral_out", &spectral_out);
+  m.def("spectral_out", &spectral_out, py::arg("U"), py::arg("h"), py::arg("Bop"), py::arg("W"), py::arg("transpose_w"),
+        py::arg("pre"), py::arg("out"), py::arg("B"), py::arg("C"), py::arg("L"), py::arg("Z"), py::arg("K1"),
+        py::arg("gelu"), py::arg("save_pre"), py::arg("pre_prev") = c10::nullopt, py::arg("h_dw") = c10::nullopt,
+        py::arg("dW") = c10::nullopt);
+  m.def("spectral_out_adj_check", &spectral_out_adj_check);
   m.def("dpre_dw", &dpre_dw);
   // limits (optional): per-digit interior bounds of a zero-padded h
   m.def("head_fwd", &head_fwd, py::arg("h"), py::arg("W3aug"), py::arg("w4b4"), py::arg("out"), py::arg("B"), py::arg("C"),

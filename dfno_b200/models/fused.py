@@ -537,10 +537,11 @@ class EnginePlan:
         return out
 
     def cost_model(self, hbm_gbs: float = H100_COPY_GBS, nvlink_gbs: Optional[float] = None,
-                   front: bool = False) -> Dict[str, object]:
+                   front: bool = False, fold_bwd: bool = False) -> Dict[str, object]:
         """Bytes every kernel of one training step must move (per rank) on this plan's routes and the resulting
         floors.  ``front``: G1a + G1b run as the single ``spectral_in`` kernel (Z1 stays on the SM); a T = 1 plan has
-        no G1b and ignores it.
+        no G1b and ignores it.  ``fold_bwd`` (round-2 route, ``num_blocks`` > 1): the backward's GELU' and bypass weight
+        gradient run inside the adjoint ``spectral_out`` (``spectral_out_adj``); ``dpre_dw`` runs for the top block only.
 
         Pure bookkeeping of the dataflow in :class:`FusedDistributedFNO` -- each stage reads its input
         buffer and writes its output buffer once; nothing is assumed to stay in L2 (the working set of a
@@ -585,9 +586,15 @@ class EnginePlan:
         else:
             # the chain's last GEMM also applies the bypass conv (+ GELU): reads U and the block input, writes the
             # pre-activation and the output (forward) / reads U and dpre, writes the input gradient (adjoint)
-            st += [("spectral_out fwd", nb, U + 3 * act, 0), ("spectral_out adj", nb, U + 2 * act, 0),
-                   ("dpre_dw", nb, 4 * act, 0),
-                   ("head fwd", 1, act + y_out, 0),
+            st += [("spectral_out fwd", nb, U + 3 * act, 0)]
+            if fold_bwd and nb > 1:
+                # top block: reads U, dpre, pre_{k-1}, writes dpre_{k-1}; middle blocks also read h_k (dW_k); block 0
+                # reads U, dpre_0, h_0 and writes g for the lift backward
+                st += [("spectral_out adj+dpre", 1, U + 3 * act, 0), ("spectral_out adj+dpre+dW", nb - 2, U + 4 * act, 0),
+                       ("spectral_out adj+dW", 1, U + 3 * act, 0), ("dpre_dw", 1, 4 * act, 0)]
+            else:
+                st += [("spectral_out adj", nb, U + 2 * act, 0), ("dpre_dw", nb, 4 * act, 0)]
+            st += [("head fwd", 1, act + y_out, 0),
                    ("head bwd", 1, 2 * act + 2 * y_out, 0)]
         hbm = sum(c * b for _, c, b, _ in st)
         link = sum(c * l for _, c, _, l in st)
@@ -827,6 +834,18 @@ class FusedDistributedFNO(nn.Module):
         # (csrc/spectral_in_sm90.cu); None where spectral_in_check refuses the shape (e.g. T > 64) -- then G1a + G1b
         # run as two dft_gemm launches -- and at T = 1, whose chain has no G1b
         self.front = self._front_plan()
+        # the backward's pointwise tail folded into the adjoint spectral_out of the block above (GELU' of block k-1,
+        # the bypass weight gradient of block k); False where spectral_out_adj_check refuses the shape (the operator
+        # and two ring stages of the middle-block variant do not fit shared memory), then dpre_dw runs for every block
+        self.fold_bwd = self._fold_bwd_plan()
+
+    def _fold_bwd_plan(self) -> bool:
+        pl = self.plan
+        if not pl.fused_pw or "iG1a_adj" not in self.ops:
+            return False
+        op = self.ops["iG1a_adj"]
+        K1 = next(st["K"] for st in self.chain_desc if st["name"] == "iG1a")
+        return not self._C.spectral_out_adj_check(op.shape[0], op.shape[1], pl.C, pl.Z, K1, True, True)
 
     @property
     def fused_pw(self) -> bool:
@@ -1015,7 +1034,8 @@ class FusedDistributedFNO(nn.Module):
             elif fuse is not None and st["name"] == "iG1a":
                 self._C.spectral_out(bufs[st["src"]], fuse["h"], self.ops[st["op"] + ("_adj" if adj else "")],
                                      fuse["W"], adj, fuse.get("pre"), dst, pl.B, pl.C, pl.X * pl.Yl * pl.T, pl.Z,
-                                     st["K"], not adj, fuse.get("pre") is not None)
+                                     st["K"], not adj, fuse.get("pre") is not None, fuse.get("pre_prev"),
+                                     fuse.get("h_dw"), fuse.get("dW"))
             else:
                 self._gemm(st, bufs, adj, add if st["name"] == "iG1a" else None)
 
@@ -1199,13 +1219,21 @@ class FusedDistributedFNO(nn.Module):
                     C_.head_bwd_multi(hs[nb], w3a, w3t, self._seg("linear4.W").view(-1), dy.contiguous().float(),
                                       self.ws["amax"], g, *head_grads, pl.B, pl.C, pl.S, pl.O, pl.Si, R, SR, *lim)
             L = pl.X * pl.Yl * pl.T
+            fold = self.fold_bwd and nb > 1
             for k in reversed(range(nb)):
                 with _nvtx(f"dfno.block{k}.bwd"):
-                    # dpre over pre (packed fp16 GELU'), bypass weight gradient reduced on the tensor core
-                    C_.dpre_dw(g, pres[k], hs[k], self._seg(f"blocks.{k}.linear.W", gf), pl.B, pl.C, L, pl.Z)
+                    fuse = dict(h=pres[k], W=self._seg(f"blocks.{k}.linear.W"))
+                    if k == nb - 1 or not fold:
+                        # dpre over pre (packed fp16 GELU'), bypass weight gradient reduced on the tensor core
+                        C_.dpre_dw(g, pres[k], hs[k], self._seg(f"blocks.{k}.linear.W", gf), pl.B, pl.C, L, pl.Z)
+                    else:
+                        # dpre_k came from the adjoint of block k+1; this adjoint forms dW_k from it and h_k
+                        fuse.update(h_dw=hs[k], dW=self._seg(f"blocks.{k}.linear.W", gf))
+                    if fold and k > 0:
+                        # ... and dpre_{k-1} = g * gelu'(pre_{k-1}) over pre_{k-1} instead of g
+                        fuse["pre_prev"] = pres[k - 1]
                     # adjoint chain; its last GEMM adds W^T dpre (the bypass input gradient) in the same accumulator
-                    self._spectral_chain(pres[k], g, k, adj=True,
-                                         fuse=dict(h=pres[k], W=self._seg(f"blocks.{k}.linear.W")), grad=gR)
+                    self._spectral_chain(pres[k], g, k, adj=True, fuse=fuse, grad=gR)
         else:
             hcl, dhb, gcl = self._saved["hcl"], self.ws["dhb"], self.ws["gcl"]
             with _nvtx("dfno.head.bwd"):

@@ -68,13 +68,13 @@ def main():
             if k != "total" and v:
                 print(f"  {k:22s} {v / 2 ** 30:9.3f} GiB")
     peaks = {"hbm": a.hbm_gbs or H100_COPY_GBS, "link": a.nvlink_gbs}
-    cm = pl.cost_model(hbm_gbs=peaks["hbm"], nvlink_gbs=peaks["link"], front=True)
+    cm = pl.cost_model(hbm_gbs=peaks["hbm"], nvlink_gbs=peaks["link"], front=True, fold_bwd=True)
     print(f"\ntraffic of one training step per rank: {cm['hbm_bytes'] / 1e9:.2f} GB HBM -> {cm['hbm_floor_ms']:.2f} ms at "
           f"{peaks['hbm']:.0f} GB/s;  {cm['nvlink_bytes'] / 1e6:.0f} MB over NVLink" +
           (f" -> {cm['nvlink_ms']:.3f} ms at {peaks['link']:.0f} GB/s (overlappable)" if peaks["link"] else
            " (no measured NVLink rate)"))
     for name, calls, hb, lb in cm["stages"]:
-        print(f"  {name:18s} x{calls:<3d} {hb / 1e9:8.3f} GB/call" + (f"  + {lb / 1e6:7.1f} MB NVLink" if lb else ""))
+        print(f"  {name:24s} x{calls:<3d} {hb / 1e9:8.3f} GB/call" + (f"  + {lb / 1e6:7.1f} MB NVLink" if lb else ""))
     print(f"\nstage chain ({'staged' if pl.staged else 'direct'} peer layout), one spectral convolution" +
           (" (G1a + G1b run as ONE kernel, spectral_in, when the shape allows: T <= 64, local Y % 4 == 0):"
            if pl.has_t else " (T_out = 1: no t stages; G1a scatters into S1, the last stage reads T1):"))
