@@ -4,7 +4,9 @@ stage of one spectral convolution -- G2, G3, iG3, iG2 and iG1b, each with the fo
 8-rank run (Yl = 64 / 32 / 16).  Every stage runs with the engine's own descriptor (EnginePlan.chain(): M, K, lda,
 ScatterSpec / ldc, column parts) into destination buffers sized as the engine sizes them; the P destination ranks of a
 multi-rank run are P buffers on this one GPU (direct T1 below 8 ranks, the staged T1s at 8).  Timed with CUDA events
-against the bytes the stage must move (its entry of EnginePlan.cost_model(front=True), per call).
+against the bytes the stage must move (its entry of EnginePlan.cost_model(front=True), per call).  A stage that runs the
+box-store epilogue (iG2 into the direct T1) is also timed with the pair scatter it replaces ("iG2 scatter", against
+the valid part of T1 that the scatter writes).
 Prints one line per stage and one JSON line; writes nothing.
 
     python benchmarks/dft_gemm_bench.py [--iters 50] [--warmup 5] [--ranks 1 2 4 8]"""
@@ -37,13 +39,18 @@ def cases(C_, P, iters, warmup, dev):
     pl = EnginePlan(1, 1, 1, BC, T, X, Y, Z, MODES, world=P, rank=0)
     pl.finish(4)
     need = {s[0]: s[2] for s in pl.cost_model(front=True)["stages"]}            # bytes per call
+    need["iG2 scatter"] = pl.n_T2 * 2 + pl.n_T1 // pl.mtp * pl.mt * 2
     ops = {k: v for k, v in pl.operators().items()}
     bufs = buffers(pl, dev)
     peers = {k: [bufs[k]] + [torch.empty_like(bufs[k]) for _ in range(P - 1)] for k in ("T1", "T1s")}
     rows = []
+    variants = []
     for st in pl.chain(staged=pl.staged):
-        if st["name"] not in STAGES:
-            continue
+        if st["name"] in STAGES:
+            variants.append((st["name"], st))
+            if "box" in st:
+                variants.append((st["name"] + " scatter", {k: v for k, v in st.items() if k != "box"}))
+    for label, st in variants:
         for adj in (False, True):
             name = st["op"] + ("_adj" if adj else "")
             A, dst = bufs[st["src"]], bufs[st["dst"]]
@@ -52,7 +59,7 @@ def cases(C_, P, iters, warmup, dev):
                 ptrs = [b.data_ptr() for b in peers[st["dst"]]] if st.get("peer_dst") else [dst.data_ptr()] * P
                 for j0, n, spec, p0, pn in pl.parts(st):
                     op = pad_operator(ops[name][2 * j0:2 * (j0 + n)], device=dev)
-                    launches.append((op, 2 * n, spec.epi(), ptrs if pn is None else ptrs[p0:p0 + pn]))
+                    launches.append((op, 2 * n, pl.epi(st, j0, n, spec), ptrs if pn is None else ptrs[p0:p0 + pn]))
             else:
                 epi = [0, 0, st["ldc"], 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 0, 0, 0, 0, 1, 0]
                 launches.append((pad_operator(ops[name], device=dev), st["N"], epi, [dst.data_ptr()]))
@@ -62,10 +69,10 @@ def cases(C_, P, iters, warmup, dev):
                     C_.dft_gemm(A, st["M"], st["K"], st["lda"], op, N, epi, ptrs, None, 0, 0)
 
             ms = time_ms(run, iters, warmup)
-            gbs = need[st["name"]] / ms / 1e6
-            rows.append({"P": P, "Yl": pl.Yl, "staged": pl.staged, "stage": st["name"], "adj": adj,
+            gbs = need[label] / ms / 1e6
+            rows.append({"P": P, "Yl": pl.Yl, "staged": pl.staged, "stage": label, "adj": adj,
                          "M": st["M"], "K": st["K"], "N": st["N"], "launches": len(launches), "ms": round(ms, 4),
-                         "bytes": need[st["name"]], "gbs": round(gbs, 1), "frac_copy": round(gbs / H100_COPY_GBS, 3)})
+                         "bytes": need[label], "gbs": round(gbs, 1), "frac_copy": round(gbs / H100_COPY_GBS, 3)})
     return rows
 
 
@@ -83,10 +90,10 @@ def main():
     for P in a.ranks:
         for r in cases(C_, P, a.iters, a.warmup, dev):
             rows.append(r)
-            print(f"P {P}  Yl {r['Yl']:3d}  {r['stage']:5s} {'adj' if r['adj'] else 'fwd'}  M {r['M']:8d}  K {r['K']:3d}  "
+            print(f"P {P}  Yl {r['Yl']:3d}  {r['stage']:11s} {'adj' if r['adj'] else 'fwd'}  M {r['M']:8d}  K {r['K']:3d}  "
                   f"N {r['N']:3d}  {r['ms']:8.3f} ms  {r['bytes'] / 1e9:6.3f} GB  {r['gbs']:7.1f} GB/s  "
                   f"{r['frac_copy']:5.1%} of copy")
-        step = [r for r in rows if r["P"] == P]
+        step = [r for r in rows if r["P"] == P and not r["stage"].endswith(" scatter")]
         print(f"P {P}  all stages, forward + adjoint chain per block x 4 blocks: "
               f"{4 * sum(r['ms'] for r in step):.3f} ms per step")
     state = gpu_state()

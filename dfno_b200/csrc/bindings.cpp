@@ -23,6 +23,7 @@ void check(const char* err, const char* what) {
 }
 
 // epi = [mode, out_fp32, ldc, nrl, R0..R3, SR0..SR3, J0, J1, SJ0, SJ1, peer_sel, peer_lvl, peer_div, base_off]
+// EPI_BOX_STORE appends the box geometry: [..., mt, mtp, kzl, KZ, Yl, y0, bcx, base_off] (dft_gemm.h, BoxGeom)
 void dft_gemm(const at::Tensor& A, int64_t M, int64_t K, int64_t lda, const at::Tensor& Bmat, int64_t N,
               const std::vector<int64_t>& epi, const std::vector<int64_t>& peer_ptrs,
               const c10::optional<at::Tensor>& add_src, int64_t ld_add, int64_t max_ctas,
@@ -30,7 +31,8 @@ void dft_gemm(const at::Tensor& A, int64_t M, int64_t K, int64_t lda, const at::
   TORCH_CHECK(A.is_cuda() && A.scalar_type() == (a_f16 ? at::kHalf : at::kBFloat16), "A must be a CUDA bf16 (or, with a_f16, fp16) tensor");
   TORCH_CHECK(Bmat.is_cuda() && Bmat.scalar_type() == at::kBFloat16 && Bmat.dim() == 2 && Bmat.is_contiguous(),
               "operator must be a contiguous CUDA bf16 [n_pad, k_pad] tensor");
-  TORCH_CHECK(epi.size() == 20, "epi descriptor must have 20 entries");
+  const bool boxed = !epi.empty() && epi[0] == dfno::EPI_BOX_STORE;
+  TORCH_CHECK(epi.size() == (boxed ? 28u : 20u), "epi descriptor must have 20 entries (28 for the box store)");
   TORCH_CHECK(!peer_ptrs.empty() && peer_ptrs.size() <= 8, "1..8 peer pointers");
   c10::cuda::CUDAGuard guard(A.device());
   dfno::GemmParams p{};
@@ -65,9 +67,16 @@ void dft_gemm(const at::Tensor& A, int64_t M, int64_t K, int64_t lda, const at::
     for (int i = 0; i + 1 < e.nrl; ++i) TORCH_CHECK(e.R[i] > 0, "row radix must be positive");
     if (e.peer_sel != dfno::PEER_NONE) TORCH_CHECK(e.peer_div > 0, "peer_div must be positive");
   }
+  dfno::BoxGeom box{};
+  if (boxed) {
+    box.mt = static_cast<int>(epi[20]); box.mtp = static_cast<int>(epi[21]); box.kzl = static_cast<int>(epi[22]);
+    box.KZ = static_cast<int>(epi[23]); box.Yl = static_cast<int>(epi[24]); box.y0 = static_cast<int>(epi[25]);
+    box.bcx = epi[26]; box.base_off = epi[27];
+  }
   int ctas = sm_count();
   if (max_ctas > 0 && max_ctas < ctas) ctas = static_cast<int>(max_ctas);
-  check(dfno::dft_gemm_launch(A.data_ptr(), lda, Bmat.data_ptr(), p, ctas, cur_stream()), "dft_gemm");
+  check(dfno::dft_gemm_launch(A.data_ptr(), lda, Bmat.data_ptr(), p, ctas, cur_stream(), boxed ? &box : nullptr),
+        "dft_gemm");
 }
 
 }  // namespace

@@ -5,7 +5,7 @@
 
 namespace dfno {
 
-enum EpiMode { EPI_ROWMAJOR = 0, EPI_PAIR_SCATTER = 1, EPI_HEAD = 2 };
+enum EpiMode { EPI_ROWMAJOR = 0, EPI_PAIR_SCATTER = 1, EPI_HEAD = 2, EPI_BOX_STORE = 3 };
 enum PeerSel { PEER_NONE = 0, PEER_BY_ROW = 1, PEER_BY_COL = 2 };
 
 // Output addressing of the epilogue.  All strides/offsets are in *elements of the output
@@ -20,6 +20,7 @@ enum PeerSel { PEER_NONE = 0, PEER_BY_ROW = 1, PEER_BY_COL = 2 };
 //   EPI_HEAD         : projection head: out[addr(row)] = s0 + sum_j v1[j] * gelu(acc[row, j] + v0[j])
 //                      (fp32 out; addr(row) from the row digits), i.e. linear3 -> gelu -> linear4
 //                      without ever materialising the 128-channel intermediate (SURVEY.md K17).
+//   EPI_BOX_STORE    : T1 box stores of the inverse y-DFT, addressed by BoxGeom (below); peers[] as above.
 struct EpiParams {
   int mode;
   int out_fp32;
@@ -56,9 +57,20 @@ struct GemmParams {
   EpiParams epi;
 };
 
+// EPI_BOX_STORE (the inverse y-DFT into T1): rows are (bcx, kz, kt), kt fastest, mt rows per kz group and kzl groups
+// per bcx (M = bcx * kzl * mt); pair j is y.  A tile holds G = tile rows / mt whole kz groups of one bcx, staged in
+// shared memory as [y][kz][kt (pitch mtp, pad words zero)] and stored with one TMA box per destination buffer:
+// pair j goes to peers[j / ybox] at T1[bcx, y0 + j % ybox, kz, kt] with T1 = peer + base_off elements,
+// [bcx][Yl][KZ][mtp] complex pairs (the rank's own kzl-wide kz slab starts at base_off).  ybox = min(N / 2, Yl).
+struct BoxGeom {
+  int mt, mtp, kzl, KZ, Yl, y0;
+  long long bcx, base_off;
+};
+
 // Returns nullptr on success, else a static error string.  `Bmat` is the operator, bf16
 // [n_pad, k_pad] row-major with zero padding; A is bf16 [M, K] with row pitch lda elements.
+// `box` describes the T1 box store and is read for p.epi.mode == EPI_BOX_STORE only.
 const char* dft_gemm_launch(const void* A, long long lda, const void* Bmat, GemmParams p, int num_sms,
-                            cudaStream_t stream);
+                            cudaStream_t stream, const BoxGeom* box = nullptr);
 
 }  // namespace dfno

@@ -37,6 +37,21 @@ struct SmemLayout {
   uint32_t stage_pitch;   // bytes per staged row (+16 B pad); 0 = direct stores
 };
 
+// EPI_BOX_STORE (dft_gemm.h, BoxGeom): per-launch state of the T1 box stores.  The other instantiations take a
+// 4-byte placeholder in its place and compile to the SASS they had without it (an empty, 1-byte-aligned parameter
+// made ptxas load the SmemLayout before it byte by byte).
+static constexpr int kMaxBoxPeers = 8;
+template <bool kBox> struct BoxArgs { int unused; };
+template <> struct alignas(64) BoxArgs<true> {
+  CUtensorMap m[kMaxBoxPeers];   // per destination, 4-byte words: dims {kzl mtp, Yl, bcx}, box {G mtp, ybox, 1}
+  int mt, mtp, G, kzl;
+  int tpb;                       // tiles per bcx: ceil(kzl / G)
+  int tiles;                     // bcx * tpb
+  int npeers, ybox, y0;
+  uint32_t peer_bytes;           // staging bytes of one destination: ybox * G * mtp words, rounded up to 128 B
+  uint32_t group_bytes;          // staging bytes of one consumer warpgroup: npeers * peer_bytes
+};
+
 // floor(n / d) for n < 2^31 with a host-computed magic number
 __device__ __forceinline__ uint32_t fast_div(uint32_t n, unsigned long long magic, int shift) {
   return static_cast<uint32_t>((static_cast<unsigned long long>(n) * magic) >> shift);
@@ -69,10 +84,12 @@ __device__ __forceinline__ long long row_offset(const EpiParams& e, uint32_t r, 
 // Accumulator fragment (sm90_ptx.cuh, wgmma D layout): thread (warp q of its warpgroup, lane l) holds, in m64 half h
 // and for i = 0, 1, the tile row 64h + 16q + l/4 + 8i; register h * kN/2 + 4j + 2i + {0, 1} is column 8j + 2(l%4) + {0, 1}
 // of that row, i.e. the (re, im) pair 4j + l%4.
-template <int kN>
+// kBox: the EPI_BOX_STORE instantiation (tiles of whole kz groups, box-stored from a staging tile); the others run
+// every other epilogue on 64 * kHalves-row tiles.
+template <int kN, bool kBox>
 __global__ void __launch_bounds__(128 * dft_max_groups(kN) + 32, 1)
 dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                const GemmParams p, const SmemLayout L) {
+                const GemmParams p, const SmemLayout L, const __grid_constant__ BoxArgs<kBox> bx) {
   constexpr int kHalves = dft_halves(kN);
   constexpr int kTileM = 64 * kHalves;
   constexpr int kAcc = dft_acc_regs(kN);
@@ -95,11 +112,30 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int lane = threadIdx.x & 31;
   const int kblocks = p.k_pad / kBlockK;
   const int kbs = static_cast<int>(L.kbs);
-  const int num_tiles = static_cast<int>((p.M + kTileM - 1) / kTileM);
+  int num_tiles;
+  if constexpr (kBox) num_tiles = bx.tiles;
+  else num_tiles = static_cast<int>((p.M + kTileM - 1) / kTileM);
+  // first A row of a tile: G whole kz groups of one bcx (box store), else 64 * kHalves consecutive rows
+  auto tile_row0 = [&](int tile) -> int {
+    if constexpr (kBox) {
+      const int bcx = tile / bx.tpb;
+      return (bcx * bx.kzl + (tile - bcx * bx.tpb) * bx.G) * bx.mt;
+    } else {
+      return tile * kTileM;
+    }
+  };
 
+  if constexpr (kBox) {
+    // the staging tiles' pad words (kt = mt .. mtp-1) are never written by the fragments: zero them once
+    uint4* z = reinterpret_cast<uint4*>(smem + L.stage_off);
+    for (uint32_t i = threadIdx.x; i < E * bx.group_bytes / 16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
+    fence_proxy_async_smem();
+  }
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if constexpr (kBox)
+      for (int j = 0; j < bx.npeers; ++j) tma_prefetch_desc(&bx.m[j]);
     for (int s = 0; s < E * spg; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 1);
@@ -128,7 +164,7 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           mbar_arrive_expect_tx(&full[s], L.a_tile_bytes);
           uint8_t* dst = smem_a + s * L.a_tile_bytes;
           for (int kb = 0; kb < kbs; ++kb)
-            tma_load_2d(dst + kb * (kTileM * 128), &tmA, &full[s], (kb0 + kb) * kBlockK, tile * kTileM);
+            tma_load_2d(dst + kb * (kTileM * 128), &tmA, &full[s], (kb0 + kb) * kBlockK, tile_row0(tile));
         }
       }
     }
@@ -143,7 +179,11 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     // per-CTA lookup tables (all consumer threads; named barrier 1)
     const int et = threadIdx.x;
     const int nthr = 128 * E;
-    if (p.epi.mode == EPI_PAIR_SCATTER) {
+    if constexpr (kBox) {
+      // pair -> word offset of its y block in the staging tile (one 128-byte aligned part per destination)
+      for (int j = et; j < npairs && j < 128; j += nthr)
+        s_coloff[j] = (j / bx.ybox) * (bx.peer_bytes / 4) + (j % bx.ybox) * bx.G * bx.mtp;
+    } else if (p.epi.mode == EPI_PAIR_SCATTER) {
       for (int j = et; j < npairs && j < 128; j += nthr) {
         int jj = j, peer = 0;
         if (p.epi.peer_sel == PEER_BY_COL) { peer = jj / p.epi.peer_div; jj -= peer * p.epi.peer_div; }
@@ -161,6 +201,16 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const uint32_t b_addr = smem_u32(smem_b);
   const int quad = lane & 3;
   float acc[kAcc];
+  // box store: word offset of this thread's fragment rows (kz, kt) inside a y block of the staging tile; rows past
+  // the tile's G kz groups are computed and dropped (-1)
+  int box_roff[kRows];
+  if constexpr (kBox) {
+#pragma unroll
+    for (int r = 0; r < kRows; ++r) {
+      const int rl = 64 * (r >> 1) + 16 * q + (lane >> 2) + 8 * (r & 1);
+      box_roff[r] = rl < bx.G * bx.mt ? (rl / bx.mt) * bx.mtp + rl % bx.mt : -1;
+    }
+  }
   uint32_t slot = 0, ph = 0;
   for (int tile = blockIdx.x + g * gridDim.x; tile < num_tiles; tile += E * gridDim.x) {
     for (int kb0 = 0; kb0 < kblocks; kb0 += kbs) {
@@ -176,7 +226,35 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     // tile row of this thread's fragment row r = 2h + i, and its row in the warp's staging slab
     auto frag_row = [&](int r) { return 64 * (r >> 1) + 16 * q + (lane >> 2) + 8 * (r & 1); };
 
-    if (p.epi.mode == EPI_ROWMAJOR && L.stage_pitch != 0) {
+    if constexpr (kBox) {
+      // ---- box store: fragments -> staging [y][kz][kt] (4-byte (re, im) words) -> one TMA box per destination,
+      // clipped at kzl and Yl; every global run is G * mtp whole words of T1
+      uint8_t* stg = smem + L.stage_off + g * bx.group_bytes;
+      const bool leader = (threadIdx.x & 127) == 0;
+      if (leader) tma_store_wait_read();                      // the previous tile's boxes have left the staging
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");
+#pragma unroll
+      for (int j = 0; j < kN / 8; ++j) {
+        const int jp = 4 * j + quad;
+        if (jp >= npairs) continue;
+        uint32_t* col = reinterpret_cast<uint32_t*>(stg) + s_coloff[jp];
+#pragma unroll
+        for (int r = 0; r < kRows; ++r) {
+          if (box_roff[r] < 0) continue;
+          const float* a = acc + (r >> 1) * kHalfRegs + 4 * j + 2 * (r & 1);
+          col[box_roff[r]] = pack_bf16x2(a[0], a[1]);
+        }
+      }
+      fence_proxy_async_smem();
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");
+      if (leader) {
+        const int bcx = tile / bx.tpb;
+        const int kz0 = (tile - bcx * bx.tpb) * bx.G;
+        for (int pj = 0; pj < bx.npeers; ++pj)
+          tma_store_3d(&bx.m[pj], stg + pj * bx.peer_bytes, kz0 * bx.mtp, bx.y0, bcx);
+        tma_store_commit();
+      }
+    } else if (p.epi.mode == EPI_ROWMAJOR && L.stage_pitch != 0) {
       // ---- coalesced row-major store: fragments -> staging rows in smem (a private slab per warp holding its
       // 16 * kHalves rows: slab row 16h + r' = tile row 64h + 16q + r') -> groups of lanes write whole rows contiguously
       uint8_t* slab = smem + L.stage_off + (warp * 32) * L.stage_pitch;
@@ -307,11 +385,19 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       const bool by_col = p.epi.peer_sel == PEER_BY_COL;
       uint64_t rbase[kRows];
       bool rok[kRows];
+#ifdef DFNO_IG2_PROBE
+      const int probe_gap = p.epi.nrl >= 2 && p.epi.SR[0] == 2 ? static_cast<int>(p.epi.SR[1] / 2) - p.epi.R[0] : 0;
+      const int probe_pad = probe_gap >= 1 && probe_gap <= 3 ? probe_gap : 0;
+      bool probe_last[kRows];
+#endif
 #pragma unroll
       for (int r = 0; r < kRows; ++r) {
         const long long row = tile0 + frag_row(r);
         int rpeer;
         rok[r] = row < p.M;
+#ifdef DFNO_IG2_PROBE
+        probe_last[r] = row % p.epi.R[0] == p.epi.R[0] - 1;
+#endif
         const long long roff = row_offset(p.epi, static_cast<uint32_t>(rok[r] ? row : 0), rpeer);
         rbase[r] = (by_col ? 0ull : reinterpret_cast<uint64_t>(p.epi.peers[rpeer])) + 2ull * roff;
       }
@@ -326,6 +412,12 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           if (!rok[r]) continue;
           const float* a = acc + (r >> 1) * kHalfRegs + 4 * j + 2 * (r & 1);
           *reinterpret_cast<uint32_t*>(rbase[r] + cadd) = pack_bf16x2(a[0], a[1]);
+#ifdef DFNO_IG2_PROBE
+          // timing builds only: the row of the last kt of a kt-padded T1 run (1..3 pad words between the row digit
+          // of radix mt and that of pitch mtp) also writes the pad words as zeros, so that every run is written whole
+          if (probe_pad > 0 && probe_last[r])
+            for (int k = 1; k <= probe_pad; ++k) *reinterpret_cast<uint32_t*>(rbase[r] + cadd + 4ull * k) = 0u;
+#endif
         }
       }
     } else {
@@ -354,7 +446,15 @@ dft_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       }
     }
   }
-  if (p.epi.peer_sel != PEER_NONE) __threadfence_system();   // publish peer stores
+  if constexpr (kBox) {
+    // the boxes must be written, not only read out of shared memory, before the fence that publishes them
+    if ((threadIdx.x & 127) == 0) {
+      tma_store_wait_all();
+      __threadfence_system();
+    }
+  } else if (p.epi.peer_sel != PEER_NONE) {
+    __threadfence_system();   // publish peer stores
+  }
 }
 
 // -------------------------------------------------------------------------------------------
@@ -368,22 +468,86 @@ static void magic_for(unsigned d, unsigned long long* magic, int* shift) {
 }
 
 // one instantiation per padded operator width (the host dispatches once per launch)
-template <int kN>
+template <int kN, bool kBox>
 static const char* launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, const SmemLayout& L,
-                          int grid, int E, uint32_t smem_bytes, cudaStream_t stream) {
+                          const BoxArgs<kBox>& bx, int grid, int E, uint32_t smem_bytes, cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(dft_gemm_kernel<kN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+    if (cudaFuncSetAttribute(dft_gemm_kernel<kN, kBox>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) !=
+        cudaSuccess)
       return "cudaFuncSetAttribute(max dynamic smem) failed";
     attr_set = true;
   }
-  dft_gemm_kernel<kN><<<grid, 128 * E + 32, smem_bytes, stream>>>(tmA, tmB, p, L);
+  dft_gemm_kernel<kN, kBox><<<grid, 128 * E + 32, smem_bytes, stream>>>(tmA, tmB, p, L, bx);
   const cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
+template <bool kBox>
+static const char* dispatch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, const SmemLayout& L,
+                            const BoxArgs<kBox>& bx, int grid, int E, uint32_t smem_bytes, cudaStream_t stream) {
+  switch (p.n_pad) {
+    case 16: return launch<16>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 32: return launch<32>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 48: return launch<48>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 64: return launch<64>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 80: return launch<80>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 96: return launch<96>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 112: return launch<112>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 128: return launch<128>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 144: return launch<144>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 160: return launch<160>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 176: return launch<176>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 192: return launch<192>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 208: return launch<208>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 224: return launch<224>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    case 240: return launch<240>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+    default: return launch<256>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+  }
+}
+
+// Box-store geometry of one launch (dft_gemm.h, BoxGeom) and its destination maps; nullptr or an error string.
+static const char* box_setup(const GemmParams& p, const BoxGeom& b, uint32_t tile_m, BoxArgs<true>* bx) {
+  const int npairs = p.N / 2;
+  if (b.mt < 1 || b.kzl < 1 || b.KZ < b.kzl || b.Yl < 1 || b.bcx < 1 || b.y0 < 0 || b.base_off < 0)
+    return "box store: bad geometry";
+  if (b.bcx * b.kzl * b.mt != p.M) return "box store: M must be bcx * kzl * mt rows";
+  if (b.mtp % 4 || b.mtp < b.mt) return "box store: the kt pitch must be a multiple of 4, at least mt";
+  bx->mt = b.mt; bx->mtp = b.mtp; bx->kzl = b.kzl;
+  bx->G = static_cast<int>(tile_m) / b.mt;
+  if (bx->G < 1) return "box store: a kz group is longer than a tile";
+  bx->tpb = (b.kzl + bx->G - 1) / bx->G;
+  if (b.bcx * bx->tpb > (1ll << 31) - 1) return "box store: too many tiles for one launch";
+  bx->tiles = static_cast<int>(b.bcx * bx->tpb);
+  bx->ybox = npairs < b.Yl ? npairs : b.Yl;
+  bx->npeers = npairs / bx->ybox;
+  bx->y0 = b.y0;
+  if (npairs % bx->ybox || bx->npeers > kMaxBoxPeers || bx->ybox > 256 || b.y0 + bx->ybox > b.Yl)
+    return "box store: the pairs must be whole destinations, or lie inside one";
+  bx->peer_bytes = (static_cast<uint32_t>(bx->ybox) * bx->G * b.mtp * 4 + 127) / 128 * 128;
+  bx->group_bytes = bx->npeers * bx->peer_bytes;
+  // the G kz groups of one (bcx, y) are one contiguous run of G * mtp words: the box's inner row
+  if (bx->G * b.mtp > 256) return "box store: more than 256 words per y in a tile";
+  PFN_encodeTiled enc = get_encode_fn();
+  if (!enc) return "cuTensorMapEncodeTiled not available";
+  cuuint64_t dims[3] = {static_cast<cuuint64_t>(b.kzl) * b.mtp, static_cast<cuuint64_t>(b.Yl),
+                        static_cast<cuuint64_t>(b.bcx)};
+  cuuint64_t str[2] = {static_cast<cuuint64_t>(b.KZ) * b.mtp * 4, static_cast<cuuint64_t>(b.Yl) * b.KZ * b.mtp * 4};
+  cuuint32_t box[3] = {static_cast<cuuint32_t>(bx->G * b.mtp), static_cast<cuuint32_t>(bx->ybox), 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  for (int j = 0; j < bx->npeers; ++j) {
+    uint8_t* base = reinterpret_cast<uint8_t*>(p.epi.peers[j]) + 2 * b.base_off;
+    if (reinterpret_cast<uintptr_t>(base) % 16) return "box store: destination must be 16B aligned";
+    if (enc(&bx->m[j], CU_TENSOR_MAP_DATA_TYPE_UINT32, 3, base, dims, str, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) !=
+        CUDA_SUCCESS)
+      return "cuTensorMapEncodeTiled(box store) failed";
+  }
+  return nullptr;
+}
+
 const char* dft_gemm_launch(const void* A, long long lda, const void* Bmat, GemmParams p, int num_sms,
-                            cudaStream_t stream) {
+                            cudaStream_t stream, const BoxGeom* box) {
   if (p.M <= 0) return nullptr;
   if (p.a_f16) return "fp16 A with a bf16 operator needs a mixed-format MMA, which sm_90 does not have";
   if (p.n_pad % 16 || p.n_pad < 16 || p.n_pad > 256) return "n_pad must be a multiple of 16 in [16,256]";
@@ -402,6 +566,12 @@ const char* dft_gemm_launch(const void* A, long long lda, const void* Bmat, Gemm
   }
   const int halves = p.n_pad <= 128 ? 2 : 1;
   const uint32_t tile_m = 64u * halves;
+  const bool boxed = p.epi.mode == EPI_BOX_STORE;
+  BoxArgs<true> bx{};
+  if (boxed) {
+    if (box == nullptr) return "box store without its geometry";
+    if (const char* err = box_setup(p, *box, tile_m, &bx)) return err;
+  }
   SmemLayout L;
   const int kblocks = p.k_pad / kBlockK;
   L.b_bytes = static_cast<uint32_t>(kblocks) * p.n_pad * 128;
@@ -412,12 +582,13 @@ const char* dft_gemm_launch(const void* A, long long lda, const void* Bmat, Gemm
       p.N == 64 || p.N == 128 || p.N == 256))
     pitch = ((p.N + 15) / 16 * 16) * (p.epi.out_fp32 ? 4 : 2) + 16;   // whole 16-column chunks are staged
   // consumer warpgroups, staging, ring depth and K chunk: as many warpgroups as the accumulator allows with >= 2
-  // stages each, whole-K stages if possible, else the largest divisor of the K blocks that leaves room for two
+  // stages each, whole-K stages if possible, else the largest divisor of the K blocks that leaves room for two.  The
+  // box store cannot run without its staging tiles (one per warpgroup).
   bool ok = false;
   int E = dft_max_groups(p.n_pad);
   for (; E >= 1 && !ok; --E) {
-    for (int with_stage = pitch ? 1 : 0; with_stage >= 0 && !ok; --with_stage) {
-      const uint32_t stg = with_stage ? 4u * E * 32 * pitch : 0;
+    for (int with_stage = (pitch || boxed) ? 1 : 0; with_stage >= (boxed ? 1 : 0) && !ok; --with_stage) {
+      const uint32_t stg = with_stage ? E * (boxed ? bx.group_bytes : 4u * 32 * pitch) : 0;
       if (fixed + stg > 227 * 1024) continue;
       const uint32_t avail = 227 * 1024 - fixed - stg;
       for (int dv = kblocks; dv >= 1 && !ok; --dv) {
@@ -439,7 +610,8 @@ const char* dft_gemm_launch(const void* A, long long lda, const void* Bmat, Gemm
   if (!ok) return "operator too large for shared memory";
   for (int l = 0; l < 4; ++l) magic_for(static_cast<unsigned>(p.epi.R[l] > 0 ? p.epi.R[l] : 1), &p.epi.Rm[l], &p.epi.Rs[l]);
   magic_for(static_cast<unsigned>(p.epi.peer_div > 0 ? p.epi.peer_div : 1), &p.epi.Pm, &p.epi.Ps);
-  const uint32_t smem_bytes = L.stage_off + (L.stage_pitch ? 4u * E * 32 * L.stage_pitch : 0);
+  const uint32_t smem_bytes =
+      L.stage_off + (boxed ? E * bx.group_bytes : L.stage_pitch ? 4u * E * 32 * L.stage_pitch : 0);
 
   CUtensorMap tmA, tmB;
   // A: the K tail beyond p.K (up to k_pad) and the M tail are zero-filled by TMA
@@ -450,26 +622,10 @@ const char* dft_gemm_launch(const void* A, long long lda, const void* Bmat, Gemm
                   static_cast<uint64_t>(p.k_pad), kBlockK, static_cast<uint32_t>(p.n_pad)))
     return "cuTensorMapEncodeTiled(B) failed";
 
-  const int num_tiles = static_cast<int>((p.M + tile_m - 1) / tile_m);
+  const int num_tiles = boxed ? bx.tiles : static_cast<int>((p.M + tile_m - 1) / tile_m);
   const int grid = num_tiles < num_sms ? num_tiles : num_sms;
-  switch (p.n_pad) {
-    case 16: return launch<16>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 32: return launch<32>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 48: return launch<48>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 64: return launch<64>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 80: return launch<80>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 96: return launch<96>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 112: return launch<112>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 128: return launch<128>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 144: return launch<144>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 160: return launch<160>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 176: return launch<176>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 192: return launch<192>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 208: return launch<208>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 224: return launch<224>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    case 240: return launch<240>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-    default: return launch<256>(tmA, tmB, p, L, grid, E, smem_bytes, stream);
-  }
+  if (boxed) return dispatch<true>(tmA, tmB, p, L, bx, grid, E, smem_bytes, stream);
+  return dispatch<false>(tmA, tmB, p, L, BoxArgs<false>{}, grid, E, smem_bytes, stream);
 }
 
 }  // namespace dfno

@@ -39,7 +39,7 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from ..ops import operators as OPS
-from ..ops.gemm import DFT_GEMM_SMEM, ScatterSpec, dft_gemm_fits, dft_gemm_min_smem, pad_operator
+from ..ops.gemm import DFT_GEMM_SMEM, BoxSpec, ScatterSpec, dft_gemm_fits, dft_gemm_min_smem, pad_operator
 from ..parallel.decomposition import balanced_bounds
 from ..parallel.partition import Partition
 
@@ -399,7 +399,11 @@ class EnginePlan:
         interleaving directly into the consumer layout (64- / 40-byte runs per destination row)
         every source rank deposits its contribution as long contiguous runs into a per-source
         block of a staging buffer (``S1s`` / ``T1s``, >= 512-byte runs), and a tiny local
-        permutation (``permS1`` / ``permT1``) produces the K-major layout of the next stage."""
+        permutation (``permS1`` / ``permT1``) produces the K-major layout of the next stage.
+
+        The direct iG2 into the kt-padded ``T1`` also carries ``box`` (a :class:`BoxSpec`) when every column part
+        of it fits the box-store epilogue (:meth:`iG2_box`); its ``scatter`` stays the model of where each pair
+        lands."""
         BC, X, Y, Z, T = self.BC, self.X, self.Y, self.Z, self.T
         Yl, KX, KY, KZ, kzl, mt, mtp = self.Yl, self.KX, self.KY, self.KZ, self.kzl, self.mt, self.mtp
         P, r = self.world, self.rank
@@ -456,13 +460,17 @@ class EnginePlan:
                            scatter=ScatterSpec(rows=[(KY, 2), (m_loc, KY * 2), (BC, X * m_loc * KY * 2)],
                                                cols=(X, m_loc * KY * 2, 0))))
         if not staged:
-            st.append(dict(name="iG2", src="T2" if self.has_x else "S4", dst="T1", M=BC * X * m_loc, K=2 * KY,
-                           lda=2 * KY, N=2 * Y, op="iG2",
-                           scatter=ScatterSpec(rows=[(mt, 2), (kzl, mtp * 2), (X, Yl * KZ * mtp * 2),
-                                                     (BC, X * Yl * KZ * mtp * 2)],
-                                               cols=(Yl, KZ * mtp * 2, 0), peer=("col", Yl),
-                                               base_off=r * kzl * mtp * 2),
-                           peer_dst=True, barrier_after=True))
+            ig2 = dict(name="iG2", src="T2" if self.has_x else "S4", dst="T1", M=BC * X * m_loc, K=2 * KY,
+                       lda=2 * KY, N=2 * Y, op="iG2",
+                       scatter=ScatterSpec(rows=[(mt, 2), (kzl, mtp * 2), (X, Yl * KZ * mtp * 2),
+                                                 (BC, X * Yl * KZ * mtp * 2)],
+                                           cols=(Yl, KZ * mtp * 2, 0), peer=("col", Yl),
+                                           base_off=r * kzl * mtp * 2),
+                       peer_dst=True, barrier_after=True)
+            box = self.iG2_box(ig2)
+            if box is not None:
+                ig2["box"] = box
+            st.append(ig2)
         else:
             st.append(dict(name="iG2", src="T2" if self.has_x else "S4", dst="T1s", M=BC * X * m_loc, K=2 * KY,
                            lda=2 * KY, N=2 * Y, op="iG2",
@@ -483,6 +491,26 @@ class EnginePlan:
         st.append(dict(name="iG1a", src="U" if self.has_t else "T1", dst="dst", M=BC * X * Yl * T, K=2 * KZ,
                        lda=2 * KZ, N=Z, op="iG1a", ldc=Z))
         return st
+
+    def iG2_box(self, st: dict) -> Optional[BoxSpec]:
+        """The box store of the direct iG2 stage ``st`` (into ``T1`` with its kt pitch ``mtp``), or None where the pair
+        scatter runs: at T = 1 (no kt axis: T1's rows are already whole words of U) and where a column part's staging
+        tile does not fit shared memory (e.g. mt = 1 with 64-row tiles: 64 kz groups of 4-word runs per y)."""
+        if not self.has_t:
+            return None
+        box = BoxSpec(self.mt, self.mtp, self.kzl, self.KZ, self.Yl, self.BC * self.X,
+                      self.rank * self.kzl * self.mtp * 2)
+        try:
+            parts = self.parts(st)
+        except ValueError:
+            return None
+        ok = all(box.column_part(j0, n)[0].fits(n, st["K"]) for j0, n, _, _, _ in parts)
+        return box if ok else None
+
+    def epi(self, st: dict, j0: int, n: int, spec: ScatterSpec) -> List[int]:
+        """Epilogue descriptor of the column part ``(j0, n, spec)`` of ``parts(st)``: the box store where the stage
+        has one, else the part's pair scatter."""
+        return st["box"].column_part(j0, n)[0].epi() if "box" in st else spec.epi()
 
     def parts(self, st: dict) -> List[Tuple[int, int, Optional[ScatterSpec], int, Optional[int]]]:
         """Column parts of one GEMM stage: ``[(j0, n_pairs, spec, first_peer, n_peers)]``.  A stage
@@ -561,10 +589,12 @@ class EnginePlan:
         Z1, S1, S2, S3, T2, U = (self.n_Z1 * bf, self.n_S1 * bf, self.n_S2 * bf, self.n_S3 * bf, self.n_T2 * bf,
                                  self.n_U * bf)
         T1 = self.n_T1 // self.mtp * self.mt * bf                      # valid (kt < mt) part
+        # iG2's box store writes whole kt-padded runs of T1 (its pad words as zeros), the pair scatter the valid part
+        T1w = self.n_T1 * bf if any("box" in s for s in self.chain(staged=self.staged)) else T1
         W = self.C * self.C * self.Q * 2 * f32                         # one block's spectral shard
         off = (P - 1) / P if P > 1 else 0.0
         chain = [("G1a", act + Z1, 0), ("G1b", Z1 + S1, S1 * off), ("G2", S1 + S2, 0), ("G3", S2 + S3, 0),
-                 ("iG3", S3 + T2, 0), ("iG2", T2 + T1, T1 * off), ("iG1b", T1 + U, 0)]
+                 ("iG3", S3 + T2, 0), ("iG2", T2 + T1w, T1w * off), ("iG1b", T1 + U, 0)]
         if not self.has_t:      # T == 1: G1a writes S1 (across NVLink), the last stage reads T1, spectral_in never runs
             U = T1
             chain = [("G1a", act + S1, S1 * off)] + chain[2:-1]
@@ -993,8 +1023,8 @@ class FusedDistributedFNO(nn.Module):
             else:
                 ptrs = [dst.data_ptr()] * max(self.world, 1)
             for j0, n, spec, p0, pn in self.plan.parts(st):
-                self._C.dft_gemm(A, st["M"], st["K"], st["lda"], self._operator(name, j0, n), 2 * n, spec.epi(),
-                                 ptrs if pn is None else ptrs[p0:p0 + pn], None, 0, 0)
+                self._C.dft_gemm(A, st["M"], st["K"], st["lda"], self._operator(name, j0, n), 2 * n,
+                                 self.plan.epi(st, j0, n, spec), ptrs if pn is None else ptrs[p0:p0 + pn], None, 0, 0)
         else:
             epi = [0, 0, st["ldc"], 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 0, 0, 0, 0, 1, 0]
             self._C.dft_gemm(A, st["M"], st["K"], st["lda"], self.ops[name], st["N"], epi, [dst.data_ptr()], add,

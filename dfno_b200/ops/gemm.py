@@ -7,9 +7,10 @@ import torch
 
 from . import build
 
-__all__ = ["pad_operator", "dft_gemm_min_smem", "dft_gemm_fits", "gemm_rowmajor", "gemm_scatter", "ScatterSpec"]
+__all__ = ["pad_operator", "dft_gemm_min_smem", "dft_gemm_fits", "gemm_rowmajor", "gemm_scatter", "ScatterSpec",
+           "BoxSpec"]
 
-EPI_ROWMAJOR, EPI_PAIR_SCATTER = 0, 1
+EPI_ROWMAJOR, EPI_PAIR_SCATTER, EPI_BOX_STORE = 0, 1, 3
 PEER_NONE, PEER_BY_ROW, PEER_BY_COL = 0, 1, 2
 
 
@@ -120,6 +121,65 @@ class ScatterSpec:
             peer, j = j // self.peer[1], j % self.peer[1]
         J0, SJ0, SJ1 = self.cols
         return peer, off + (j % J0) * SJ0 + (j // J0) * SJ1
+
+
+class BoxSpec:
+    """Box-store epilogue of the inverse y-DFT into ``T1`` (``EPI_BOX_STORE``, ``csrc/dft_gemm_sm90.cu``).
+
+    The rows of A are ``(bcx, kz, kt)``, kt fastest: ``mt`` rows per kz group, ``kzl`` groups per bcx, ``bcx`` = B*C*X
+    row blocks.  A tile takes ``G = tile_rows // mt`` whole kz groups of one bcx (rows past them are computed and
+    dropped), stages them in shared memory as ``[y][kz][kt (pitch mtp)]`` with zero pad words, and leaves as one TMA
+    box per destination buffer.  Pair ``j`` (= y) goes to buffer ``j // ybox`` at ``T1[bcx, y0 + j % ybox, kz, kt]``,
+    ``T1`` = that buffer + ``base_off`` bf16 elements with ``[bcx][Yl][KZ][mtp]`` complex pairs; ``ybox = min(n, Yl)``
+    for a launch of ``n`` pairs.  Every global run is ``G * mtp`` whole pairs, clipped at ``kzl`` and ``Yl``."""
+
+    def __init__(self, mt: int, mtp: int, kzl: int, KZ: int, Yl: int, bcx: int, base_off: int, y0: int = 0):
+        self.mt, self.mtp, self.kzl, self.KZ, self.Yl = mt, mtp, kzl, KZ, Yl
+        self.bcx, self.base_off, self.y0 = bcx, base_off, y0
+
+    def epi(self) -> List[int]:
+        return [EPI_BOX_STORE] + [0] * 19 + [self.mt, self.mtp, self.kzl, self.KZ, self.Yl, self.y0, self.bcx,
+                                             self.base_off]
+
+    def column_part(self, j0: int, n: int) -> Tuple["BoxSpec", int, Optional[int]]:
+        """The launch of pairs ``[j0, j0+n)``: ``(spec, first_peer, n_peers)`` as :meth:`ScatterSpec.column_part`
+        returns them for the pair scatter of the same stage (whole destinations, or a y range inside one)."""
+        Yl = self.Yl
+        if j0 % Yl == 0 and n % Yl == 0:
+            return BoxSpec(self.mt, self.mtp, self.kzl, self.KZ, Yl, self.bcx, self.base_off), j0 // Yl, n // Yl
+        if Yl % n == 0 and j0 % n == 0:
+            return (BoxSpec(self.mt, self.mtp, self.kzl, self.KZ, Yl, self.bcx, self.base_off, j0 % Yl), j0 // Yl, 1)
+        raise ValueError(f"cannot split {n} pairs at {j0} over destinations of {Yl}")
+
+    @staticmethod
+    def tile_rows(n: int) -> int:
+        """Rows of one dft_gemm tile for a launch of ``n`` pairs (64 when the operator is wider than 128 rows)."""
+        return 64 if _ceil(2 * n, 16) > 128 else 128
+
+    def groups(self, n: int) -> int:
+        """kz groups per tile (``G``)."""
+        return self.tile_rows(n) // self.mt
+
+    def tiles(self, n: int) -> List[Tuple[int, int]]:
+        """``(first row, live rows)`` of every tile, in launch order (the kernel's tile -> row mapping)."""
+        G = self.groups(n)
+        tpb = -(-self.kzl // G)
+        return [((b * self.kzl + c * G) * self.mt, min(G, self.kzl - c * G) * self.mt)
+                for b in range(self.bcx) for c in range(tpb)]
+
+    def fits(self, n: int, K: int) -> bool:
+        """Can one launch of ``n`` pairs and reduction length ``K`` take the box store?  Mirrors ``box_setup`` and
+        the shared-memory sizing of ``dft_gemm_launch``: the resident operator, barriers and tables, and for every
+        consumer warpgroup the accumulator allows (2 or 3) a ring of two 64-wide K blocks and one staging tile.  With
+        fewer warpgroups a tile's box would have to leave before the next tile's staging starts, so shapes whose
+        staging crowds them out (mt = 1 at 128 y: 64 kz groups of 4-word runs per y, 128 KB) keep the pair scatter."""
+        G, ybox = self.groups(n), min(n, self.Yl)
+        if G < 1 or G * self.mtp > 256 or ybox > 256 or n % ybox or n // ybox > 8 or self.mtp % 4:
+            return False
+        n_pad, tile = _ceil(2 * n, 16), self.tile_rows(n)
+        groups = 3 if (tile // 64) * n_pad // 2 <= 64 else 2
+        stg = n // ybox * _ceil(ybox * G * self.mtp * 4, 128)
+        return n_pad * _ceil(K, 64) * 2 + 5120 + groups * (stg + 2 * tile * 128) <= DFT_GEMM_SMEM
 
 
 def gemm_scatter(A: torch.Tensor, M: int, K: int, lda: int, Bpad: torch.Tensor, N: int,
