@@ -295,21 +295,31 @@ __device__ __forceinline__ void wg_mma64(float (&acc)[R], int n, uint64_t da, ui
 // K loop runs out of (uniform) registers for the descriptors and is serialised too.  The block loop is a run-time
 // loop with a fence per block; ptxas closes it with one extra arrive before the wait (C7519).
 // `accumulate`: add to the accumulator instead of overwriting it (the second and later K chunks of one tile).
-template <int N, int kHalves, int R>
-__device__ __forceinline__ void mma_chain(float (&acc)[R], uint32_t a, uint32_t a_blk, uint32_t b, uint32_t b_blk,
-                                          int kblocks, bool accumulate = false) {
+// mma_issue is the chain without its commit and wait, so that several chains into one accumulator share them.  kTB = 1
+// takes B MN-major instead (N <= 64: one 128-byte atom along N, rows of 128 bytes along K, so a k16 step is 16 rows
+// = 2048 bytes and b_blk = 8192 per K block).
+template <int N, int kHalves, int kTB, int R>
+__device__ __forceinline__ void mma_issue(float (&acc)[R], uint32_t a, uint32_t a_blk, uint32_t b, uint32_t b_blk,
+                                          int kblocks, bool accumulate) {
+  static_assert(kTB == 0 || N <= 64, "an MN-major B operand is one atom wide");
   int kb = 0;
 #pragma unroll 1
   do {
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
-      const uint64_t da = gdesc_k128(a + kb * a_blk + kk * 32), db = gdesc_k128(b + kb * b_blk + kk * 32);
+      const uint64_t da = gdesc_k128(a + kb * a_blk + kk * 32);
+      const uint64_t db = kTB ? gdesc_mn128(b + kb * b_blk + kk * 2048, 16384, 1024) : gdesc_k128(b + kb * b_blk + kk * 32);
       const uint32_t scale_d = accumulate || kb > 0 || kk > 0 ? 1u : 0u;
-      wg_mma64<false, 0, 0, 0>(acc, N, da, db, scale_d);
-      if constexpr (kHalves == 2) wg_mma64<false, 0, 0, R / 2>(acc, N, da + (8192 >> 4), db, scale_d);
+      wg_mma64<false, 0, kTB, 0>(acc, N, da, db, scale_d);
+      if constexpr (kHalves == 2) wg_mma64<false, 0, kTB, R / 2>(acc, N, da + (8192 >> 4), db, scale_d);
     }
   } while (++kb < kblocks);
+}
+template <int N, int kHalves, int R>
+__device__ __forceinline__ void mma_chain(float (&acc)[R], uint32_t a, uint32_t a_blk, uint32_t b, uint32_t b_blk,
+                                          int kblocks, bool accumulate = false) {
+  mma_issue<N, kHalves, 0>(acc, a, a_blk, b, b_blk, kblocks, accumulate);
   wgmma_commit();
   wgmma_wait<0>();
   acc_fence(acc);

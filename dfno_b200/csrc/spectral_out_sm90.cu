@@ -15,10 +15,15 @@
 //                                               output, used as an MN-major operand (z contiguous), so the
 //                                               channel mixing is a contraction over the tile's own rows
 //
-// The epilogue thread of row m owns a whole z-line: it rounds the accumulator to bf16 (pre-activation,
-// kept for the backward), evaluates the GELU in packed fp16 and hands both tiles to TMA stores through a
-// swizzled staging buffer.  The activation is therefore read once (as B2) and written once per layer; the
-// separate bypass+GELU pass of round 1 (4 more activation passes per block) is gone.
+// Tiles are 64 columns (one swizzle block) of R lines x C channels, so every operand is one 16 KB box and a stage is
+// {U (k1blocks boxes), h}.  The owner warpgroup of a tile (tiles alternate) issues MMA1 and MMA2 as one chain of
+// compile-time width (the tile's padded column count, chosen once per tile: a width chosen per instruction makes
+// ptxas serialise every wgmma, C7511) into an m128 x n64 accumulator, and runs the epilogue on its fragments: each
+// thread rounds its adjacent-column pairs to bf16 (pre) and through the packed fp16 GELU (out), and writes them as
+// 4-byte words of the swizzled tile (conflict-free) -- pre over the h slot, out over the first U block, both dead once
+// the chain has completed and both of the output's box geometry -- from where a store warp TMA-stores them and,
+// once the stores have read the stage, releases it (waiting for that read in the consumers held them up for every
+// tile).  The activation is therefore read once (as B2) and written once per layer.
 #include "sm90_ptx.cuh"
 #include "kernels.h"
 #include "tma_host.h"
@@ -27,23 +32,56 @@ namespace dfno {
 namespace {
 
 constexpr uint32_t kBlk = 16384;          // one [128 rows][64 bf16] SWIZZLE_128B block
-constexpr int kMaxStagesS = 4;
+constexpr int kMaxStagesS = 6;
 constexpr int kMaxE = 2;                  // consumer warpgroups (stages a multiple of E: see bypass_sm90.cu)
 
 struct SpecOutParams {
   int B, C, R, RC;
   long long L;              // lines per (b, c)
   long long tiles_per_b;    // ceil(L / R)
-  int Z, nzt;               // row length; column tiles of up to 128 columns
+  int Z, nzt;               // row length; column tiles of up to 64 columns
   int K1, k1blocks, n_pad;  // DFT operator: reduction length, 64-wide K blocks, rows in memory
   int transpose_w;
   const float* W;           // [C, C] fp32
   int stages, E;
-  uint32_t stage_bytes, zbt;
+  uint32_t stage_bytes;
 };
 
+// MMA1 + MMA2 of one tile into an m128 x nN accumulator, issued back to back (the caller commits and waits):
+//   MMA1   D  = U tile . F^T            (both K-major; every K block, the tail past K1 is zero-filled by TMA)
+//   MMA2   D += (W (x) I_R) . B2 tile   (B MN-major: z contiguous; both 64-row blocks, rows >= R*C are zero)
+template <int N>
+__device__ __forceinline__ void out_mmas(float (&acc)[64], uint32_t a1, uint32_t b1, uint32_t b1_blk, int k1blocks,
+                                         uint32_t a2, uint32_t b2) {
+  mma_issue<N, 2, 0>(acc, a1, kBlk, b1, b1_blk, k1blocks, false);
+  mma_issue<N, 2, 1>(acc, a2, kBlk, b2, 8192, 2, true);
+}
+// One dispatch per tile on its padded column count ntp (16, 32, 48 or 64)
+__device__ __forceinline__ void out_mmas_n(int ntp, float (&acc)[64], uint32_t a1, uint32_t b1, uint32_t b1_blk,
+                                           int k1blocks, uint32_t a2, uint32_t b2) {
+  switch (ntp) {
+    case 16: out_mmas<16>(acc, a1, b1, b1_blk, k1blocks, a2, b2); break;
+    case 32: out_mmas<32>(acc, a1, b1, b1_blk, k1blocks, a2, b2); break;
+    case 48: out_mmas<48>(acc, a1, b1, b1_blk, k1blocks, a2, b2); break;
+    default: out_mmas<64>(acc, a1, b1, b1_blk, k1blocks, a2, b2); break;
+  }
+}
+
+// A2 = W (x) I_R (or W^T (x) I_R) as two K-major 64-column blocks: row m = (a, r), column k = (b, r)
+__device__ __forceinline__ void build_a2(uint8_t* s_a2, const SpecOutParams& p, bool transpose) {
+  for (int idx = threadIdx.x; idx < p.C * p.C * p.R; idx += blockDim.x) {
+    const int a = idx / (p.C * p.R);                  // output channel (row block)
+    const int rem = idx - a * (p.C * p.R);
+    const int b = rem / p.R, r = rem - b * p.R;       // input channel (column block), line inside the tile
+    const float w = transpose ? p.W[b * p.C + a] : p.W[a * p.C + b];
+    const int m = a * p.R + r, k = b * p.R + r;
+    const uint32_t off = (k >> 6) * kBlk + m * 128 + (((((k & 63) >> 3) ^ (m & 7)) << 4) | ((k & 7) << 1));
+    *reinterpret_cast<__nv_bfloat16*>(s_a2 + off) = __float2bfloat16(w);
+  }
+}
+
 template <bool kGelu, bool kPre>
-__global__ void __launch_bounds__(128 * kMaxE + 32, 1)
+__global__ void __launch_bounds__(128 * kMaxE + 64, 1)
 spectral_out_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmH,
                     const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmP,
                     const __grid_constant__ CUtensorMap tmO, const SpecOutParams p) {
@@ -51,17 +89,17 @@ spectral_out_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_consta
   uint8_t* s_b1 = smem;
   uint8_t* s_a2 = s_b1 + static_cast<uint32_t>(p.k1blocks) * p.n_pad * 128;
   uint8_t* s_ring = s_a2 + 2 * kBlk;
-  uint8_t* s_stage = s_ring + p.stages * p.stage_bytes;
-  float* s_scratch = reinterpret_cast<float*>(s_stage + p.E * p.zbt * kBlk);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_scratch + 4 * p.E * kRowScratchFloats);
-  uint64_t* full = bars;              // [4] TMA -> consumer
-  uint64_t* empty = bars + 4;         // [4] consumer -> TMA
-  uint64_t* bfull = bars + 8;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_ring + p.stages * p.stage_bytes);
+  uint64_t* full = bars;                        // [kMaxStagesS] TMA -> consumer
+  uint64_t* empty = bars + kMaxStagesS;         // [kMaxStagesS] store warp -> TMA
+  uint64_t* done = bars + 2 * kMaxStagesS;      // [kMaxStagesS] consumer -> store warp
+  uint64_t* bfull = bars + 3 * kMaxStagesS;
+  const uint32_t o_h = p.k1blocks * kBlk;       // stage slots: U blocks, then h
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const long long num_tiles = p.tiles_per_b * p.B * p.nzt;
 
-  // rows >= R*C of every operand block are never written by TMA: zero them once; build A2 = W (x) I_R
+  // rows >= R*C of every operand block are never written by TMA (nor by the epilogue): zero them once; build A2
   {
     uint4* z0 = reinterpret_cast<uint4*>(s_a2);
     const uint32_t nz = (2 * kBlk + p.stages * p.stage_bytes) / 16;
@@ -70,20 +108,12 @@ spectral_out_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_consta
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmU); tma_prefetch_desc(&tmH); tma_prefetch_desc(&tmB1);
     tma_prefetch_desc(&tmP); tma_prefetch_desc(&tmO);
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); mbar_init(&done[s], 1); }
     mbar_init(bfull, 1);
     fence_barrier_init();
   }
   __syncthreads();
-  for (int idx = threadIdx.x; idx < p.C * p.C * p.R; idx += blockDim.x) {
-    const int a = idx / (p.C * p.R);                  // output channel (row block)
-    const int rem = idx - a * (p.C * p.R);
-    const int b = rem / p.R, r = rem - b * p.R;       // input channel (column block), line inside the tile
-    const float w = p.transpose_w ? p.W[b * p.C + a] : p.W[a * p.C + b];
-    const int m = a * p.R + r, k = b * p.R + r;
-    const uint32_t off = (k >> 6) * kBlk + m * 128 + (((((k & 63) >> 3) ^ (m & 7)) << 4) | ((k & 7) << 1));
-    *reinterpret_cast<__nv_bfloat16*>(s_a2 + off) = __float2bfloat16(w);
-  }
+  build_a2(s_a2, p, p.transpose_w != 0);
   fence_proxy_async_smem();
   __syncthreads();
 
@@ -94,113 +124,90 @@ spectral_out_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_consta
       for (int kb = 0; kb < p.k1blocks; ++kb) tma_load_2d(s_b1 + kb * p.n_pad * 128, &tmB1, bfull, kb * 64, 0);
       uint32_t s = 0, ph = 0;
       for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int zt = static_cast<int>(tile % p.nzt);
+        const int zb = static_cast<int>(tile % p.nzt);
         const long long lt = (tile / p.nzt) % p.tiles_per_b;
         const int b = static_cast<int>(tile / (p.nzt * p.tiles_per_b));
-        const int ncols = min(128, p.Z - zt * 128);
-        const int zbn = (ncols + 63) >> 6;
-        mbar_wait(&empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&full[s], static_cast<uint32_t>(p.k1blocks + zbn) * p.RC * 128);
-        uint8_t* dst = s_ring + s * p.stage_bytes;
         const int l0 = static_cast<int>(lt * p.R);
+        mbar_wait(&empty[s], ph ^ 1);
+        mbar_arrive_expect_tx(&full[s], static_cast<uint32_t>(p.k1blocks + 1) * p.RC * 128);
+        uint8_t* dst = s_ring + s * p.stage_bytes;
         for (int kb = 0; kb < p.k1blocks; ++kb) tma_load_3d(dst + kb * kBlk, &tmU, &full[s], kb * 64, l0, b * p.C);
-        for (int zb = 0; zb < zbn; ++zb)
-          tma_load_3d(dst + (p.k1blocks + zb) * kBlk, &tmH, &full[s], zt * 128 + zb * 64, l0, b * p.C);
+        tma_load_3d(dst + o_h, &tmH, &full[s], zb * 64, l0, b * p.C);
         if (++s == static_cast<uint32_t>(p.stages)) { s = 0; ph ^= 1; }
       }
     }
     return;
   }
+  if (warp == 4 * p.E + 1) {
+    // ===================== store warp: the finished tiles' TMA stores, then the stage goes back to the producer =====
+    // (waiting here for the stores to have read the stage keeps that latency off the consumer warpgroups)
+    if (lane == 0) {
+      long long n = 0;
+      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
+        const uint32_t s = static_cast<uint32_t>(n % p.stages);
+        const int zb = static_cast<int>(tile % p.nzt);
+        const long long lt = (tile / p.nzt) % p.tiles_per_b;
+        const int b = static_cast<int>(tile / (p.nzt * p.tiles_per_b));
+        const int l0 = static_cast<int>(lt * p.R);
+        uint8_t* st = s_ring + s * p.stage_bytes;
+        mbar_wait(&done[s], (n / p.stages) & 1);
+        if (kPre) tma_store_3d(&tmP, st + o_h, zb * 64, l0, b * p.C);
+        tma_store_3d(&tmO, st, zb * 64, l0, b * p.C);
+        tma_store_commit();
+        tma_store_wait_read();
+        mbar_arrive(&empty[s]);
+      }
+      tma_store_wait_all();
+    }
+    return;
+  }
 
-  // ===================== consumer warpgroups: both MMAs, then the epilogue (one thread per row (c, r)) =========
+  // ===================== consumer warpgroups: the chain, then the epilogue on the fragments =====================
   const int q = warp & 3, g = warp >> 2;
-  const int m = wg_row128(q, lane);
   const bool t0 = q == 0 && lane == 0;
-  uint8_t* stg = s_stage + g * p.zbt * kBlk;
-  uint8_t* myrow = stg + m * 128;
-  float* scratch = s_scratch + warp * kRowScratchFloats;
-  const uint32_t sw = m & 7;
   const uint32_t barid = 1 + g;
-  const int k1steps = (p.K1 + 15) >> 4;
-  const int k2steps = (p.RC + 15) >> 4;
   const uint32_t b1_addr = smem_u32(s_b1), a2_addr = smem_u32(s_a2);
-  mbar_wait(bfull, 0);
-  float acc[128];
+  mbar_wait_warp(bfull, 0);
+  float acc[64];
   long long n = 0;
   for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
     if (n % p.E != g) continue;
     const uint32_t s = static_cast<uint32_t>(n % p.stages);
-    const int zt = static_cast<int>(tile % p.nzt);
-    const long long lt = (tile / p.nzt) % p.tiles_per_b;
-    const int b = static_cast<int>(tile / (p.nzt * p.tiles_per_b));
-    const int ncols = min(128, p.Z - zt * 128);
-    const int ntp = (ncols + 15) & ~15;
-    const int zbn = (ncols + 63) >> 6;
-    const int l0 = static_cast<int>(lt * p.R);
-    mbar_wait(&full[s], (n / p.stages) & 1);
-    {
-      //   MMA1   D  = U tile . F^T          (both K-major)
-      //   MMA2   D += (W (x) I_R) . h tile   (B MN-major: z contiguous, atoms every kBlk bytes along z)
-      const uint32_t a1 = smem_u32(s_ring + s * p.stage_bytes);
-      const uint32_t b2 = a1 + p.k1blocks * kBlk;
-      const uint32_t b1 = b1_addr + zt * 128 * 128;
-      wgmma_fence();
-      for (int ks = 0; ks < k1steps; ++ks) {
-        const uint32_t kb = ks >> 2, kk = ks & 3;
-        wg_mma128<false, 0, 0>(acc, ntp, gdesc_k128(a1 + kb * kBlk + kk * 32), 8192,
-                               gdesc_k128(b1 + kb * (p.n_pad * 128) + kk * 32), ks > 0 ? 1u : 0u);
-      }
-      for (int ks = 0; ks < k2steps; ++ks) {       // K = the tile's own rows (c, r): 16 rows per instruction
-        const uint32_t kb = ks >> 2, kk = ks & 3;
-        wg_mma128<false, 0, 1>(acc, ntp, gdesc_k128(a2_addr + kb * kBlk + kk * 32), 8192,
-                               gdesc_mn128(b2 + ks * 2048, kBlk, 1024), 1u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      acc_fence(acc);
-      if (t0) mbar_arrive(&empty[s]);                  // the ring stage may be refilled
-    }
-    if (t0) tma_store_wait_read();                     // the previous tile's stores have left the staging buffer
-    asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
-    // accumulator -> bf16 (the pre-activation, or the GELU of it when `act`) -> swizzled staging rows
-    auto stage_rows = [&](bool act) {
+    const int zb = static_cast<int>(tile % p.nzt);
+    const int ncols = min(64, p.Z - zb * 64);
+    uint8_t* st = s_ring + s * p.stage_bytes;
+    const uint32_t a1 = smem_u32(st);
+    mbar_wait_warp(&full[s], (n / p.stages) & 1);
+    out_mmas_n((ncols + 15) & ~15, acc, a1, b1_addr + zb * 64 * 128, p.n_pad * 128, p.k1blocks, a2_addr, a1 + o_h);
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(acc);
+    asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");   // every warp's MMAs have read the stage
+    // register h*32 + 4j + e holds row 64h + 16q + lane/4 + 8(e/2), columns 8j + 2(lane%4) + {0, 1}: the same
+    // adjacent-column pairs a row view pairs, so pre and the packed GELU round exactly as they would there
 #pragma unroll
-      for (int ch = 0; ch < 8; ++ch) {
-        const int c0 = ch * 16;
-        if (c0 < ncols) {
-          uint32_t v[16], pk[8];
-          wg_row16<2>(acc, c0, scratch, v);
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float x0 = __uint_as_float(v[2 * i]), x1 = __uint_as_float(v[2 * i + 1]);
-            pk[i] = act ? h2_to_bf16x2(gelu_h2(h2_from_f32(x0, x1))) : pack_bf16x2(x0, x1);
+      for (int eh = 0; eh < 2; ++eh) {
+        const int m = 64 * h + 16 * q + (lane >> 2) + 8 * eh;
+        if (m < p.RC) {                               // rows >= R*C of the slots stay zero: they are MMA operands
+          uint8_t* row = st + m * 128 + 4 * (lane & 3);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            if (8 * j < ncols) {
+              const float* a = acc + 32 * h + 4 * j + 2 * eh;
+              const uint32_t off = (j ^ (m & 7)) << 4;
+              if (kPre) *reinterpret_cast<uint32_t*>(row + o_h + off) = pack_bf16x2(a[0], a[1]);
+              *reinterpret_cast<uint32_t*>(row + off) =
+                  kGelu ? h2_to_bf16x2(gelu_h2(h2_from_f32(a[0], a[1]))) : pack_bf16x2(a[0], a[1]);
+            }
           }
-          uint8_t* rowp = myrow + (c0 >> 6) * kBlk;
-          const uint32_t j0 = (c0 & 63) >> 3;
-          *reinterpret_cast<uint4*>(rowp + ((j0 ^ sw) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          *reinterpret_cast<uint4*>(rowp + (((j0 + 1) ^ sw) << 4)) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
         }
       }
-      fence_proxy_async_smem();
-      asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
-    };
-    stage_rows(kGelu && !kPre);
-    if (t0) {
-      const CUtensorMap* mp = kPre ? &tmP : &tmO;
-      for (int zb = 0; zb < zbn; ++zb) tma_store_3d(mp, stg + zb * kBlk, zt * 128 + zb * 64, l0, b * p.C);
-      tma_store_commit();
-    }
-    if (kPre) {                                      // the GELU of the same accumulator, after the pre store left
-      if (t0) tma_store_wait_read();
-      asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
-      stage_rows(true);
-      if (t0) {
-        for (int zb = 0; zb < zbn; ++zb) tma_store_3d(&tmO, stg + zb * kBlk, zt * 128 + zb * 64, l0, b * p.C);
-        tma_store_commit();
-      }
-    }
+    fence_proxy_async_smem();
+    asm volatile("bar.sync %0, 128;" ::"r"(barid) : "memory");
+    if (t0) mbar_arrive(&done[s]);                   // the tile is in the stage: over to the store warp
   }
-  if (t0) tma_store_wait_all();
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -225,6 +232,15 @@ spectral_out_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_consta
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kAdjE = 2;
 
+// Rows 64g .. 64g + 63 of the weight-gradient D += dpre_k . h_k^T over one tile (both K-major, K = the tile's 64
+// columns; columns past Z are zero-filled in both slots, so all four k16 steps run): one chain, the caller fences
+// before it and commits after it.  `first`: the CTA's first tile overwrites the accumulator.
+__device__ __forceinline__ void dw_mmas(float (&accw)[64], uint32_t d, uint32_t h, bool first) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk)
+    wgmma_m64n128k16_bf16<0, 0>(accw, gdesc_k128(d + kk * 32), gdesc_k128(h + kk * 32), (!first || kk > 0) ? 1u : 0u);
+}
+
 template <bool kDpre, bool kDw>
 __global__ void __launch_bounds__(128 * kAdjE + 32, 1)
 spectral_out_adj_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmD,
@@ -235,9 +251,9 @@ spectral_out_adj_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_co
   uint8_t* s_a2 = s_b1 + static_cast<uint32_t>(p.k1blocks) * p.n_pad * 128;
   uint8_t* s_ring = s_a2 + 2 * kBlk;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_ring + p.stages * p.stage_bytes);
-  uint64_t* full = bars;              // [4] TMA -> consumers
-  uint64_t* empty = bars + 4;         // [4] consumers -> TMA
-  uint64_t* bfull = bars + 8;
+  uint64_t* full = bars;                        // [kMaxStagesS] TMA -> consumers
+  uint64_t* empty = bars + kMaxStagesS;         // [kMaxStagesS] consumers -> TMA
+  uint64_t* bfull = bars + 2 * kMaxStagesS;
   // stage slots: U blocks, then dpre_k, pre_{k-1}, h_k
   const uint32_t o_d = p.k1blocks * kBlk, o_p = o_d + kBlk, o_h = o_p + (kDpre ? kBlk : 0);
 
@@ -257,15 +273,7 @@ spectral_out_adj_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_co
     fence_barrier_init();
   }
   __syncthreads();
-  for (int idx = threadIdx.x; idx < p.C * p.C * p.R; idx += blockDim.x) {   // A2 = W^T (x) I_R
-    const int a = idx / (p.C * p.R);
-    const int rem = idx - a * (p.C * p.R);
-    const int b = rem / p.R, r = rem - b * p.R;
-    const float w = p.W[b * p.C + a];
-    const int m = a * p.R + r, k = b * p.R + r;
-    const uint32_t off = (k >> 6) * kBlk + m * 128 + (((((k & 63) >> 3) ^ (m & 7)) << 4) | ((k & 7) << 1));
-    *reinterpret_cast<__nv_bfloat16*>(s_a2 + off) = __float2bfloat16(w);
-  }
+  build_a2(s_a2, p, true);                      // A2 = W^T (x) I_R
   fence_proxy_async_smem();
   __syncthreads();
 
@@ -298,8 +306,6 @@ spectral_out_adj_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_co
   const int q = warp & 3, g = warp >> 2;
   const bool t0 = q == 0 && lane == 0;
   const uint32_t barid = 1 + g;
-  const int k1steps = (p.K1 + 15) >> 4;
-  const int k2steps = (p.RC + 15) >> 4;
   const uint32_t b1_addr = smem_u32(s_b1), a2_addr = smem_u32(s_a2);
   mbar_wait(bfull, 0);
   float acc[64];                      // D[m, z] of the tiles this warpgroup owns (m128 x n64)
@@ -312,7 +318,6 @@ spectral_out_adj_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_co
     const long long lt = (tile / p.nzt) % p.tiles_per_b;
     const int b = static_cast<int>(tile / (p.nzt * p.tiles_per_b));
     const int ncols = min(64, p.Z - zb * 64);
-    const int ntp = (ncols + 15) & ~15;
     const int l0 = static_cast<int>(lt * p.R);
     uint8_t* st = s_ring + s * p.stage_bytes;
     const uint32_t a1 = smem_u32(st);
@@ -322,10 +327,7 @@ spectral_out_adj_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_co
       // fp16 pairs (kDpre), while the owner runs its MMAs -- the owner's epilogue then only multiplies
       if constexpr (kDw) {
         wgmma_fence();
-        const int ksteps = ntp >> 4;
-        for (int kk = 0; kk < ksteps; ++kk)
-          wgmma_m64n128k16_bf16<0, 0>(accw, gdesc_k128(a1 + o_d + g * 8192 + kk * 32), gdesc_k128(a1 + o_h + kk * 32),
-                                      (n > 0 || kk > 0) ? 1u : 0u);
+        dw_mmas(accw, a1 + o_d + g * 8192, a1 + o_h, n == 0);
         wgmma_commit();
       }
       if constexpr (kDpre) {
@@ -359,25 +361,9 @@ spectral_out_adj_kernel(const __grid_constant__ CUtensorMap tmU, const __grid_co
     {
       //   MMA1   D  = U tile . F'^T        (both K-major)
       //   MMA2   D += (W^T (x) I_R) . dpre_k tile   (B MN-major, z contiguous)
-      //   (kDw)  D[64g + (o, r), (i, r')] += dpre_k[(o, r), z] . h_k[(i, r'), z]   (K = z; columns beyond Z zero-filled)
-      wgmma_fence();
-      const uint32_t b1 = b1_addr + zb * 64 * 128;
-      for (int ks = 0; ks < k1steps; ++ks) {
-        const uint32_t kb = ks >> 2, kk = ks & 3;
-        wg_mma128<false, 0, 0>(acc, ntp, gdesc_k128(a1 + kb * kBlk + kk * 32), 8192,
-                               gdesc_k128(b1 + kb * (p.n_pad * 128) + kk * 32), ks > 0 ? 1u : 0u);
-      }
-      for (int ks = 0; ks < k2steps; ++ks) {
-        const uint32_t kb = ks >> 2, kk = ks & 3;
-        wg_mma128<false, 0, 1>(acc, ntp, gdesc_k128(a2_addr + kb * kBlk + kk * 32), 8192,
-                               gdesc_mn128(a1 + o_d + ks * 2048, kBlk, 1024), 1u);
-      }
-      if constexpr (kDw) {
-        const int ksteps = ntp >> 4;
-        for (int kk = 0; kk < ksteps; ++kk)
-          wgmma_m64n128k16_bf16<0, 0>(accw, gdesc_k128(a1 + o_d + g * 8192 + kk * 32), gdesc_k128(a1 + o_h + kk * 32),
-                                      (n > 0 || kk > 0) ? 1u : 0u);
-      }
+      //   (kDw)  D[64g + (o, r), (i, r')] += dpre_k[(o, r), z] . h_k[(i, r'), z]   (K = z)
+      out_mmas_n((ncols + 15) & ~15, acc, a1, b1_addr + zb * 64 * 128, p.n_pad * 128, p.k1blocks, a2_addr, a1 + o_d);
+      if constexpr (kDw) dw_mmas(accw, a1 + o_d + g * 8192, a1 + o_h, n == 0);
       wgmma_commit();
       wgmma_wait<0>();
       acc_fence(acc);
@@ -481,18 +467,17 @@ const char* spectral_out(const void* U, const void* h, const void* Bop, int n_pa
   SpecOutParams p{};
   p.B = B; p.C = C; p.R = 128 / C; p.RC = p.R * C; p.L = L;
   p.tiles_per_b = (L + p.R - 1) / p.R;
-  p.Z = Z; p.nzt = (Z + 127) / 128;
+  p.Z = Z; p.nzt = (Z + 63) / 64;
   p.K1 = K1; p.k1blocks = k_pad / 64; p.n_pad = n_pad;
   p.transpose_w = transpose_w; p.W = W;
-  p.zbt = Z > 64 ? 2 : 1;
-  p.stage_bytes = (p.k1blocks + p.zbt) * kBlk;
+  p.stage_bytes = (p.k1blocks + 1) * kBlk;
   const uint32_t fixed = static_cast<uint32_t>(p.k1blocks) * n_pad * 128 + 2 * kBlk + 1024 /*barriers*/ + 1024 /*align*/;
   const uint32_t budget = 227 * 1024;
-  auto scratch_bytes = [](int E) { return static_cast<uint32_t>(4 * E * kRowScratchFloats * 4); };
+  // the deepest ring that fits (4 stages of 32 KB at K1 <= 64, Z <= 128: two tiles in flight per warpgroup)
   p.E = kMaxE; p.stages = 0;
   for (int E = kMaxE; E >= 1 && !p.stages; --E)
     for (int st = kMaxStagesS; st >= 2; --st)
-      if (st % E == 0 && fixed + st * p.stage_bytes + E * p.zbt * kBlk + scratch_bytes(E) <= budget) {
+      if (st % E == 0 && fixed + st * p.stage_bytes <= budget) {
         p.E = E; p.stages = st; break;
       }
   if (!p.stages) return "spectral_out: tile does not fit shared memory";
@@ -503,10 +488,10 @@ const char* spectral_out(const void* U, const void* h, const void* Bop, int n_pa
   if (make_map_2d(&tmB1, Bop, k_pad, n_pad, k_pad, 64, n_pad)) return "tensor map (operator) failed";
   if (make_map_3d(&tmP, pre ? pre : out, Z, L, BC, Z, static_cast<uint64_t>(L) * Z, 64, p.R, C)) return "tensor map (pre) failed";
   if (make_map_3d(&tmO, out, Z, L, BC, Z, static_cast<uint64_t>(L) * Z, 64, p.R, C)) return "tensor map (out) failed";
-  const uint32_t smem_bytes = fixed + p.stages * p.stage_bytes + p.E * p.zbt * kBlk + scratch_bytes(p.E);
+  const uint32_t smem_bytes = fixed + p.stages * p.stage_bytes;
   const long long tiles = p.tiles_per_b * B * p.nzt;
   const int grid = static_cast<int>(tiles < num_sms ? tiles : num_sms);
-  const int threads = 128 * p.E + 32;
+  const int threads = 128 * p.E + 64;
   const uint32_t dyn = smem_bytes;
   const bool want_pre = gelu && save_pre && pre != nullptr;
 #define DFNO_SO_LAUNCH(G, P)                                                                                         \
